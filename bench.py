@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the Predict()/Perceive() hot path on B200 (BASELINE.json metric).
+"""bench.py — throughput of the Predict()/Perceive() hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--streams S] [--step-bytes B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--streams S] [--step-bytes B] [--dump-outputs DIR]
     python bench.py --impl reference ...           # the reference's own CPU implementation on the box's host cores
 
 Workload = BASELINE.json configs[1]: synthetic enwik8-shaped ASCII text (tools/gen_synth.py, seed 0xE9E80001),
@@ -18,6 +18,9 @@ every stream by --step-bytes bytes (8x as many coded bits). One stream = one ref
             stream, against MEASURED_PEAKS.json; `kernels` lists every bulk kernel's measured time per coded bit so that
             the share of each (and the pole) is visible.
 `bpc`       cross entropy of the coded prefix from the device's probabilities, next to the reference's on the same bytes.
+--dump-outputs DIR writes the probabilities the timed path returned in its last timed step (DIR/p.npy, float32, one row
+            per stream; DIR/p_rank<r>.npy per rank under torchrun). The inputs are seeded, so two builds run with the same
+            arguments can be compared output for output.
 Multi-GPU (torchrun): independent files per rank, no data-path collective (weak scaling); time = max over ranks.
 """
 import argparse
@@ -38,30 +41,26 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-# algorithmic bytes per coded bit (DESIGN.md §4) and ncu's DRAM bytes per coded bit of one launch (profiles/)
+# algorithmic bytes per coded bit (DESIGN.md §4)
 ALGO_BYTES_PER_BIT = {
     "mix_kernel_v3": 450_000,       # SURVEY.md §8(d): 55 172 fp32 weights read + written, + input vectors
     "paq8_kernel": 212_000,         # 28 selected int16 weight sets x 1552 read + written (174 KB) + ~273 live contexts x (64 B bucket line r/w + StateMap cells)
     "fxcm_kernel": 34_000,          # 10 selected weight rows x 512 int16 read + written (20 KB) + ~100 live contexts x 140 B
 }
-NCU_DRAM_BYTES_PER_BIT = {
-    "mix_kernel_v3": 34_786,        # profiles/r01_ncu_full_metrics.csv: (63.16 MB + 8.09 MB) / 2048 bits
-    "paq8_kernel": 22_483,          # profiles/r02_ncu_producers.txt: (22.28 MB + 0.74 MB) / 1024 bits (weight sets stay in shared memory)
-    "fxcm_kernel": 4_100,           # profiles/r02_ncu_producers.txt
-}
 KERNELS = ["mix_kernel_v3", "small_kernel", "lstm_kernel", "ppmd_kernel", "fxcm_kernel", "paq8_kernel"]
 SEED = 0xE9E80001
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def measured_hbm_peak():
     try:
         return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "fallback: H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (a read-only query)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -142,6 +141,19 @@ def cpu_baseline(n_file, sample_bytes):
             "strict_value": r_strict["bytes"] / r_strict["code_s"] / 1e6, "bpc_reference": r_strict["bpc"], "bpc_reference_fast_build": r_fast["bpc"] if r_fast else None}
 
 
+def dump_outputs(out_dir, name, rows):
+    """The caller-visible probabilities of one step (one row per stream) as float32 .npy. Above DUMP_LIMIT_BYTES a fixed,
+    seeded sample of columns is written instead, with its column indices in <name>_index.npy."""
+    p = np.stack([r.cpu().numpy() for r in rows]).astype(np.float32)
+    os.makedirs(out_dir, exist_ok=True)
+    if p.nbytes > DUMP_LIMIT_BYTES:
+        keep = DUMP_LIMIT_BYTES // (4 * p.shape[0])
+        idx = np.sort(np.random.default_rng(0).choice(p.shape[1], keep, replace=False))
+        p = p[:, idx]
+        np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, name + ".npy"), p)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -152,6 +164,7 @@ def main():
     ap.add_argument("--aggregate-streams", type=int, default=int(os.environ.get("CMIXB200_BENCH_AGG", "7")), help="files per GPU for the aggregate figure (0 = skip)")
     ap.add_argument("--step-bytes", type=int, default=1024)
     ap.add_argument("--cpu-sample-bytes", type=int, default=4096)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's probabilities to DIR/*.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -188,7 +201,7 @@ def main():
     from cmix_b200.capi import code_batch, code_batch_device
     from cmix_b200.sharding import stream_block, reduce_timing
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device - the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device - the CUDA path has no CPU fallback")
     dist = None
     if world > 1:
         if os.environ.get("NCCL_DEBUG", "VERSION").upper() == "VERSION":
@@ -273,6 +286,9 @@ def main():
     sampler.stop_flag = True
     sampler.join(timeout=2)
     value = total_bytes / dt / 1e6
+    if args.dump_outputs and K > 0:
+        dump_outputs(args.dump_outputs, "p" if world == 1 else "p_rank%d" % rank,
+                     [st["d_out"][(W + K - 1) * B * 8:(W + K) * B * 8] for st in head])
 
     # ---- end to end through the C-ABI with pinned HOST buffers: the same streams continue ----
     preds = [st["P"] for st in head]
@@ -333,7 +349,7 @@ def main():
             bits_per_launch = n_bits / n
             ach = ALGO_BYTES_PER_BIT[kname] * bits_per_launch / (ms / n / 1e3) / 1e9
             roof[kname] = {"achieved": ach, "frac": ach / peak, "launches": n, "ms_total": ms, "bits_per_launch": bits_per_launch,
-                           "algorithmic_bytes_per_bit": ALGO_BYTES_PER_BIT[kname], "traffic": NCU_DRAM_BYTES_PER_BIT[kname] * bits_per_launch}
+                           "algorithmic_bytes_per_bit": ALGO_BYTES_PER_BIT[kname]}
         dom = pole if pole in roof else "mix_kernel_v3"
         p_dev = head[0]["d_out"][W * B * 8:(W + K) * B * 8].cpu().numpy().astype(np.float64)
         bits_coded = np.unpackbits(head[0]["text"][W * B:(W + K) * B])
@@ -345,8 +361,6 @@ def main():
                     "note": "cmixb200_code_batch with pinned host buffers: the step's bytes go up and its probabilities come back inside the timed region (bytes per rank per step)"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": dom, "achieved": roof[dom]["achieved"], "peak": peak, "unit": "GB/s", "frac": roof[dom]["frac"],
-                         "traffic": roof[dom]["traffic"], "traffic_unit": "B per launch",
-                         "traffic_source": "ncu --set full DRAM read+write of one launch per coded bit (profiles/r02_ncu_producers.txt, r01_ncu_full_metrics.csv) x bits per launch",
                          "peak_source": "MEASURED_PEAKS.json (%s)" % peak_kind, "per_kernel": roof,
                          "note": "the dominant kernel is the one the stream waits for (longest CUDA-event time per coded bit). Every kernel of this path is LATENCY bound, "
                                  "not bandwidth bound: bit t+1 cannot start before bit t is perceived, the integer models walk dependent hash-bucket chains and every "

@@ -1,4 +1,4 @@
-"""cmix_b200 — B200-native per-bit context-mixing predictor behind cmix's Predictor surface.
+"""cmix_b200 — H100-native per-bit context-mixing predictor behind cmix's Predictor surface.
 
 The product is the C-ABI shared library built from cmix_b200/csrc (see include/cmixb200.h);
 this package is the thin Python binding used by tests/ and bench.py. It never falls back to

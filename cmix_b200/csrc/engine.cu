@@ -1,4 +1,4 @@
-// cmix_b200/csrc/engine.cu — host side of the B200 predictor engine + the C-ABI
+// cmix_b200/csrc/engine.cu — host side of the H100 predictor engine + the C-ABI
 // declared in include/cmixb200.h.
 //
 // Host responsibilities (everything numeric runs in the kernels):

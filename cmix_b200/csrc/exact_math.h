@@ -66,14 +66,12 @@ static inline double xm_u2d(uint64_t u) { double x; memcpy(&x, &u, 8); return x;
 #endif
 
 #if defined(__CUDACC__)
-// Two IEEE fp32 products in one issue slot (FMUL2 on sm_100a). Each half is rounded to nearest exactly
-// like a scalar FMUL, so a serial FADD chain fed by it reproduces the reference's sum bit for bit.
+// Two IEEE fp32 products, each rounded to nearest (sm_90a has no paired fp32 multiply: two FMULs).
+// The explicit rounding keeps nvcc from contracting them into the FADD chain they feed, so that
+// chain reproduces the reference's sum bit for bit.
 __device__ __forceinline__ void xm_fmul2(float ax, float ay, float bx, float by, float& px, float& py) {
-  unsigned long long a, b, r;
-  asm("mov.b64 %0, {%1,%2};" : "=l"(a) : "f"(ax), "f"(ay));
-  asm("mov.b64 %0, {%1,%2};" : "=l"(b) : "f"(bx), "f"(by));
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  asm("mov.b64 {%0,%1}, %2;" : "=f"(px), "=f"(py) : "l"(r));
+  px = __fmul_rn(ax, bx);
+  py = __fmul_rn(ay, by);
 }
 #endif
 

@@ -5,7 +5,7 @@
 // (:1622-1646), the two match models (:1742-1841, :3420-3700), the run map (:756-829) and the 429 exported 12-bit
 // codes (:97-105, SURVEY Appendix B #19). Bit-exact by construction: every quantity is an integer.
 //
-// How it is organised for the B200 (fxcm.cuh runs it; tools/fxcm_check.cpp runs the same code on the CPU):
+// How it is organised for the GPU (fxcm.cuh runs it; tools/fxcm_check.cpp runs the same code on the CPU):
 //  * ONE flat state block per stream (FxState) of offsets into HBM arenas; no pointers into tables are kept —
 //    bit-history cells are addressed by 32-bit byte offsets into their bucket table.
 //  * The per-bit work is cut into UNITS that own disjoint state and disjoint slices of the input / export vectors

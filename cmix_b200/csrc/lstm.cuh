@@ -13,7 +13,7 @@
 // ~1M independent weight elements in the weight-gradient accumulation, which is
 // restructured from "100 rank-1 updates" into one pass where each thread owns one
 // weight and adds its 100 terms in the reference's time order (99 -> 0).
-// Tensor cores are deliberately not used: tcgen05 kinds round products to
+// Tensor cores are deliberately not used: wgmma rounds fp32 operands to
 // TF32/BF16 and accumulate in an unspecified order; either breaks bit-exactness
 // (DESIGN.md §6).
 //
@@ -104,7 +104,7 @@ __device__ __forceinline__ float sum_back_to_front(const float* p, int n) {
   return s;
 }
 
-// f += sum_j a[j] * w[j * stride], j = 0..n-1 in order: one FADD chain; the products come two at a time (FMUL2),
+// f += sum_j a[j] * w[j * stride], j = 0..n-1 in order: one FADD chain; the products come two at a time (xm_fmul2),
 // the broadcast operand as LDS.128. a must be 16-byte aligned.
 __device__ __forceinline__ float chain_strided(float f, const float* a, const float* w, int n, int stride) {
   const float4* a4 = reinterpret_cast<const float4*>(a);

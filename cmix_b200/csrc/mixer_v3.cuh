@@ -14,7 +14,7 @@
 //
 // Warp roles (roles are pinned to schedulers: the arbiter prefers high warp ids):
 // * C warp (15): lanes 0..12 = the CTA's 13 layer-0 mixers. Chain out of shared memory with
-//   LDS.128 ping-pong buffers and packed FMUL2 products feeding one FADD chain per lane; then the
+//   LDS.128 ping-pong buffers and __fmul_rn products feeding one FADD chain per lane; then the
 //   triangular extra-input substitution; then u = decay*lr*(sigma(p)-bit) with decay*lr
 //   pre-computed by the movers (mixer.cpp:58-60).
 // * mover warps (11): while bit t's chains run they plan bit t+1 - stage the 2078 inputs (triple

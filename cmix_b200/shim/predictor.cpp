@@ -1,4 +1,4 @@
-// cmix_b200/shim/predictor.cpp — Predictor methods forwarding to the B200 engine.
+// cmix_b200/shim/predictor.cpp — Predictor methods forwarding to the CUDA engine.
 // Error convention of the reference: none (no return codes, no exceptions; allocation failure
 // exits, e.g. fxcmv1.cpp:142). A CUDA failure therefore prints the C-ABI error and exits(1):
 // a half-written archive is useless, and there is no CPU fallback to fall back to.

@@ -1,4 +1,4 @@
-/* include/cmixb200.h — C-ABI of the B200-native cmix predictor.
+/* include/cmixb200.h — C-ABI of the H100-native cmix predictor.
  *
  * Drop-in boundary: the reference's `class Predictor` (reference
  * src/predictor.h:17-53), the only interface the reference's arithmetic coder
@@ -9,7 +9,7 @@
  *
  * Plain pointers and sizes only; no C++ or torch types. All functions return
  * CMIXB200_OK (0) or an error code; cmixb200_last_error() describes the failure.
- * There is no CPU fallback behind any of them: without a usable sm_100 device
+ * There is no CPU fallback behind any of them: without a usable sm_90 device
  * they fail with CMIXB200_ERR_CUDA.
  */
 #ifndef CMIXB200_H

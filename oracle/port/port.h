@@ -2,10 +2,10 @@
 //
 // Plain scalar C++ restatement of the reference's Predictor::Predict/Perceive
 // path (reference src/predictor.cpp:361-487) for the rows of SURVEY.md §8(a)
-// that the B200 engine runs on the device: a1-a12 and a16-a18. The three big
+// that the CUDA engine runs on the device: a1-a12 and a16-a18. The three big
 // third-party model families (PAQ8 a13, FXCM a14, PPMD a15) are NOT restated:
 // their per-bit outputs are *replayed* from a dump produced by the real
-// reference (oracle/_ref/oracle_dump, built from /root/reference by
+// reference (oracle/_ref/oracle_dump, built from the reference checkout by
 // oracle/Makefile).
 //
 // Pinning: tests/test_oracle_port.py checks this port bit-for-bit against the

@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run on the GPU box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run on a GPU machine with -m gpu)")
 
 
 class Golden:
@@ -43,6 +43,15 @@ def golden(request):
 @pytest.fixture(scope="session")
 def golden_text():
     return Golden("text208")
+
+
+@pytest.fixture(scope="session")
+def dict_path(tmp_path_factory):
+    """The reference's WRT dictionary as a file: the C-ABI and tools/fxcm_check.cpp take a path."""
+    from gen_synth import dictionary
+    path = tmp_path_factory.mktemp("dic") / "english.dic"
+    path.write_bytes(dictionary())
+    return str(path)
 
 
 @pytest.fixture(scope="session")

@@ -1,5 +1,5 @@
 """bench.py's reference arm runs on the CPU (the unmodified reference through oracle/_ref): its JSON line must carry the keys the
-driver reads, on the same metric / unit / config as the B200 arm."""
+driver reads, on the same metric / unit / config as the GPU arm."""
 import json
 import os
 import subprocess

@@ -54,7 +54,7 @@ GOLD_1M = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "lo
 
 @pytest.mark.gpu
 @pytest.mark.timeout(3600)
-@pytest.mark.skipif(os.environ.get("CMIXB200_SLOW") != "1" or not os.path.exists(GOLD_1M), reason="1 MiB run: set CMIXB200_SLOW=1 (5 minutes on a B200)")
+@pytest.mark.skipif(os.environ.get("CMIXB200_SLOW") != "1" or not os.path.exists(GOLD_1M), reason="1 MiB run: set CMIXB200_SLOW=1")
 def test_1m_text_equals_the_reference():
     """Same check over 1 MiB (gen_synth seed 0xE9E80011): 8.4 M coded bits, one CRC per 4 096; run on demand."""
     import cmix_b200

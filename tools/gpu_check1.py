@@ -1,6 +1,7 @@
 # first GPU parity check against a dump generated on the box
 import os, sys, subprocess, time, numpy as np
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tools')
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tools'))
 from oracle_io import Dump, N_EXT
 import cmix_b200
 from gen_synth import synth_text
@@ -8,7 +9,7 @@ os.makedirs('/tmp/w', exist_ok=True)
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 1500
 open('/tmp/w/s.txt','wb').write(synth_text(n))
 t0=time.time()
-subprocess.run(['/root/repo/oracle/_ref/oracle_dump','dump','n','/tmp/w/s.txt','/tmp/w/d','2'], check=True, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+subprocess.run([os.path.join(ROOT, 'oracle', '_ref', 'oracle_dump'),'dump','n','/tmp/w/s.txt','/tmp/w/d','2'], check=True, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
 print('oracle dump took', time.time()-t0)
 d = Dump('/tmp/w/d')
 t0=time.time()

@@ -1,6 +1,7 @@
 # per-phase cycle profile of the mix kernel (clock64 counters) on synthetic replay streams
-import sys, time, numpy as np
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tests')
+import os, sys, time, numpy as np
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import cmix_b200
 from conftest import synthetic_streams
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 512

@@ -1,5 +1,6 @@
-import sys, numpy as np
-sys.path.insert(0, "/root/repo"); sys.path.insert(0, "/root/repo/tests"); sys.path.insert(0, "/root/repo/tools")
+import os, sys, numpy as np
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests")); sys.path.insert(0, os.path.join(ROOT, "tools"))
 import cmix_b200
 from conftest import synthetic_streams
 stream, vocab, codes, ppmd = synthetic_streams(40, seed=5)

@@ -37,19 +37,23 @@ def tables():
     return dict(l.split() for l in (a + b).splitlines())
 
 
+def ours(name):
+    """The hex string paq8_host.h carries for table `name` ("" when it has none)."""
+    src = open(os.path.join(ROOT, "cmix_b200", "csrc", "paq8_host.h")).read()
+    field = {"state": r"&T\.state\[0\]\[0\]"}.get(name, r"T\." + name)
+    m = re.search(r"unhex\(" + field + r", \d+,(.*?)\);", src, re.S)
+    return "".join(re.findall(r'"(.*?)"', m.group(1))) if m else ""
+
+
 def main():
     t = tables()
     if "--check" not in sys.argv:
         for k, v in t.items():
             print(k, v)
         return 0
-    src = open(os.path.join(ROOT, "cmix_b200", "csrc", "paq8_host.h")).read()
     bad = 0
     for name, want in t.items():
-        field = {"state": r"&T\.state\[0\]\[0\]"}.get(name, r"T\." + name)
-        m = re.search(r"unhex\(" + field + r", \d+,(.*?)\);", src, re.S)
-        got = "".join(re.findall(r'"(.*?)"', m.group(1))) if m else ""
-        if got != want:
+        if ours(name) != want:
             print("table", name, "differs")
             bad = 1
     return bad

@@ -1,6 +1,7 @@
 # per-phase cycle profile of the resident PPMD model (ppmd.cuh) on synthetic enwik-shaped text
-import sys, time, numpy as np
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tools')
+import os, sys, time, numpy as np
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tools'))
 import cmix_b200
 from gen_synth import synth_text
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 4096

@@ -44,7 +44,7 @@ def run(n_bytes):
     P = cmix_b200.Predictor(vocab)
     P.code_bytes(text[:n_bytes])
     lib = load_library()
-    sm_mhz = torch.cuda.get_device_properties(0).clock_rate / 1e3 if hasattr(torch.cuda.get_device_properties(0), "clock_rate") else 1965.0
+    sm_mhz = torch.cuda.get_device_properties(0).clock_rate / 1e3 if hasattr(torch.cuda.get_device_properties(0), "clock_rate") else 1980.0
     for name, fn, rows in (("paq8", "cmixb200_p8_prof", 96), ("fxcm", "cmixb200_fx_prof", 24)):
         if not hasattr(lib, fn):
             continue
