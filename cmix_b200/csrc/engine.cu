@@ -827,6 +827,15 @@ int RunPipelined(cmixb200_predictor** preds, int n_streams, const u8* const* d_b
     HarvestMixTimes(G);
   }
   if (!pretrain) for (int s = 0; s < n_streams; ++s) preds[s]->bits_done += n_bytes * 8;
+  // The bulk kernels keep the resident models' codes for the next bit in their State only; a lock-step Predict() or the
+  // decoder's first prediction reads them from d_ext_bit, so hand them over (the models' current outputs, predictor.cpp:361-369).
+  // Replayed slots keep their rule: 0.5 until fed.
+  for (int s = 0; s < n_streams; ++s) {
+    cmixb200_predictor* P = preds[s];
+    if (P->d_fx) CK(cudaMemcpyAsync(P->d_ext_bit, (const u8*)P->d_fx + offsetof(fx::State, codes), fx::N_OUT * sizeof(u16), cudaMemcpyDeviceToDevice, P->s_mix));
+    if (P->d_p8) CK(cudaMemcpyAsync(P->d_ext_bit + fx::N_OUT, (const u8*)P->d_p8 + offsetof(p8::State, codes), p8::N_OUT * sizeof(u16), cudaMemcpyDeviceToDevice, P->s_mix));
+  }
+  for (int s = 0; s < n_streams; ++s) if (preds[s]->d_fx || preds[s]->d_p8) CK(cudaStreamSynchronize(preds[s]->s_mix));   // PAQ8's next Perceive() writes on s_p8
   if (any_ppmd) {
     for (int s = 0; s < n_streams; ++s) {
       uint32_t err = 0;
