@@ -25,6 +25,12 @@
 
 #include "fxcm_text.h"
 
+// Host census of the device-only clash path (tools/census.h): called where the in-order map loop starts, with the state the
+// device's per-bit probe sees. Empty in every product build.
+#ifndef FX_CENSUS_MAP
+#define FX_CENSUS_MAP(S, id) do { } while (0)
+#endif
+
 namespace cmixb200 {
 namespace fx {
 
@@ -330,6 +336,7 @@ FX_HD inline void map_finish(State& S, int id, u32 result) {
 }
 // One bit of one context map, contexts in order (mix / mix1).
 FX_HD inline void map_bit(State& S, int id, Out& o) {
+  FX_CENSUS_MAP(S, id);
   u32 result = 0;
   const int cn = S.map[id].cn;
   for (int i = 0; i < cn; ++i) result += map_ctx_bit(S, id, i, o);

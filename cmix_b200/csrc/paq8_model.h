@@ -25,6 +25,14 @@
 #else
 #define P8_HD
 #endif
+// Host census of the device-only paths (tools/census.h): called where the in-order loops start, with the state the device's
+// per-bit probe sees. Empty in every product build.
+#ifndef P8_CENSUS_CM
+#define P8_CENSUS_CM(T, m, y, c0, bp) do { } while (0)
+#endif
+#ifndef P8_CENSUS_CM2
+#define P8_CENSUS_CM2(m, bpos) do { } while (0)
+#endif
 
 namespace cmixb200 {
 namespace p8 {
@@ -379,6 +387,7 @@ P8_HD inline int cm_step(Cm& m, int i, Out& o, int ns, int y, int c0, int bp, in
 // The in-order loop. `rnd` is the global generator: draws happen in context order.
 P8_COLD P8_HD inline int cm_mix(Cm& m, Out& o, Rnd& rnd, int y, int c0, int bp, int c1) {
   const Tables& T = *o.T;
+  P8_CENSUS_CM(T, m, y, c0, bp);
   int result = 0;
   for (int i = 0; i < m.cn; ++i) {
     int ns = cm_next_state(T, m, i, y);
@@ -569,6 +578,7 @@ P8_COLD P8_HD inline int cm2_mix_body(Cm2& m, Out& o, int y, int bpos) {   // af
 }
 P8_HD inline int cm2_mix(Cm2& m, Out& o, int y, int bpos) {
   cm2_begin(m, y, bpos);
+  P8_CENSUS_CM2(m, bpos);
   const int result = cm2_mix_body(m, o, y, bpos);
   if (bpos == 7) m.index = 0;
   return result;

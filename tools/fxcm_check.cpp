@@ -9,6 +9,7 @@
 // LSTM feedback FXCM consumed (<prefix>.lstmfx.u32). With a dictionary the reference pretrains on a 5-byte header plus
 // the dictionary text (preprocessor.cpp:37-69) before the first coded bit; so does this tool.
 // With crc_out it writes one CRC32 per 4096 bits of its OWN codes (fixture generation once the run is green).
+// Built with -DCENSUS it also prints how often the coded bits reach the device-only clash path (tools/census.h).
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -17,6 +18,9 @@
 #include <string>
 #include <vector>
 
+#ifdef CENSUS
+#include "census.h"
+#endif
 #include "fxcm_host.h"
 
 using namespace cmixb200::fx;
@@ -85,6 +89,9 @@ int main(int argc, char** argv) {
     for (unsigned char c : pre) for (int j = 7; j >= 0; --j) bit_serial(*S, (c >> j) & 1, 0, 0);
     fprintf(stderr, "pretrained on %zu bytes\n", pre.size());
   }
+#ifdef CENSUS
+  census::reset();
+#endif
 
   std::vector<uint16_t> want(2022);
   std::vector<uint32_t> crcs;
@@ -111,6 +118,9 @@ int main(int argc, char** argv) {
       crc = crc32_update(crc, S->codes, 431 * 2);
       if ((t & 4095) == 4095) { crcs.push_back(crc); crc = 0; }
       bit_serial(*S, (stream[pos] >> j) & 1, (int)(lfx[t] & 0xffff), (int)(lfx[t] >> 16));
+#ifdef CENSUS
+      census::end_bit();
+#endif
     }
   }
   if (crc_out) {
@@ -118,6 +128,9 @@ int main(int argc, char** argv) {
     fwrite(crcs.data(), 4, crcs.size(), f);
     fclose(f);
   }
+#ifdef CENSUS
+  census::print(stdout, {});
+#endif
   printf("%s: %zu bytes, %zu bits compared, %zu mismatching bits\n", bad_bits ? "FAIL" : "OK", n_bytes, n_bytes * 8, bad_bits);
   return bad_bits ? 1 : 0;
 }

@@ -8,6 +8,7 @@
 // A pretrain file holds the bytes the reference's Pretrain() saw before the first coded bit (5-byte header + dictionary
 // with '\n' -> ' ', preprocessor.cpp:37-69). With crc_out it writes one CRC32 per 4096 bits over its OWN 1591 codes.
 // first_slot/last_slot (0-based within the 1591) restrict the comparison while a sub-model range is being brought up.
+// Built with -DCENSUS it also prints how often the coded bits reach the device-only paths (tools/census.h).
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -16,6 +17,9 @@
 #include <string>
 #include <vector>
 
+#ifdef CENSUS
+#include "census.h"
+#endif
 #include "paq8_host.h"
 
 using namespace cmixb200::p8;
@@ -70,6 +74,9 @@ int main(int argc, char** argv) {
     for (unsigned char c : pre) for (int j = 7; j >= 0; --j) bit(*S, (c >> j) & 1);
     fprintf(stderr, "pretrained on %zu bytes\n", pre.size());
   }
+#ifdef CENSUS
+  census::reset();
+#endif
   std::vector<uint16_t> want(2022);
   std::vector<uint32_t> crcs;
   uint32_t crc = 0;
@@ -95,10 +102,20 @@ int main(int argc, char** argv) {
       crc = crc32_update(crc, S->codes, 1591 * 2);
       if ((t & 4095) == 4095) { crcs.push_back(crc); crc = 0; }
       bit(*S, (stream[pos] >> j) & 1);
+#ifdef CENSUS
+      census::end_bit();
+#endif
       if (S->error) { fprintf(stderr, "model raised error %u at bit %zu (unsupported block type)\n", S->error, t); printf("UNSUPPORTED after %zu bits\n", t); return 3; }
     }
   }
   if (crc_out) { FILE* f = fopen(crc_out, "wb"); fwrite(crcs.data(), 4, crcs.size(), f); fclose(f); }
+#ifdef CENSUS
+  census::print(stdout, {{"sparse", &S->sparse.cm}, {"sparse1", &S->sparse1.cm}, {"distance", &S->distance.cm}, {"record.cm", &S->record.cm},
+                         {"record.cn", &S->record.cn}, {"record.co", &S->record.co}, {"record.cp", &S->record.cp}, {"record1.cm", &S->record1.cm},
+                         {"record1.cn", &S->record1.cn}, {"record1.co", &S->record1.co}, {"record1.cq", &S->record1.cq},
+                         {"record1.cp", &S->record1.cp}, {"word", &S->word.cm}, {"nest", &S->nest.cm}, {"indirect", &S->indirect.cm},
+                         {"xml", &S->xml.cm}, {"order-n (history)", &S->cm}, {"text (history)", &S->text.map}, {"exe (history)", &S->exe.cm}});
+#endif
   printf("%s: %zu bytes, %zu mismatching bits (slots %d..%d)\n", bad_bits ? "FAIL" : "OK", n_bytes, bad_bits, first, last);
   return bad_bits ? 1 : 0;
 }
