@@ -1,6 +1,6 @@
 // cmix_b200/csrc/paq8.cuh — the resident PAQ8 model on the device (SURVEY §8 row a13).
 //
-// One CTA of 12 warps per stream evaluates paq8_top.h's `bit()` with the work of a bit spread over lanes:
+// One cluster of two CTAs per stream evaluates paq8_top.h's `bit()`; 12 warps of the first spread the models over lanes:
 //  * every context of every context map is a lane (210 lanes for the sixteen 7-slot maps on warps 0-6, 63 for the three
 //    history maps on warps 7-8): bucket probe, bit-history step, state maps and the 5 / 7 mixer inputs of a context are
 //    independent of the other contexts of its map as long as they touch different 64-byte buckets this bit. That is CHECKED
@@ -17,21 +17,31 @@
 //    the sparse and record models consume what the order-N map and the match model produce in the same bit) and the three
 //    OLS predictors (one warp each: rank-1 covariance update with coalesced columns, Cholesky with a row per lane in
 //    registers, substitutions in the reference's summation order).
-//  * the 28 selected int16 weight sets (1552 weights each) are CACHED in shared memory from the dot product of one bit to
-//    the SGD step of the next and written back to HBM only when a selector moves to another set; dot products and SGD use
-//    all 384 lanes (integer sums: exact under any association).
-// The 55 KB state block, the hot read-only tables (21 KB) and the 87 KB weight cache live in shared memory for the launch;
-// the ~10 GB of model memory stays in HBM.
+//  * the mixer and the SSE stage run one or more bits behind the models on a second CTA of a 2-CTA cluster (nothing the
+//    models compute reads them back: the mixer's output feeds only the SSE stage, `st_misses` and selector set 26). The
+//    model CTA (rank 0) hands each bit over through a ring of P8_RING slots in the mixer CTA's shared memory (inputs,
+//    their codes, the 28 selectors, the SSE context), one full / one empty mbarrier per slot, and blocks only when the
+//    ring is full. The mixer CTA (rank 1) trains the sets picked for bit t-1 on its inputs as soon as bit t is known,
+//    then runs bit t's 28 dot products, the final mixer and the SSE stage, and writes the 1591-code rows.
+//  * the 28 selected int16 weight sets (1552 weights each) are CACHED in the mixer CTA's shared memory from the dot product
+//    of one bit to the SGD step of the next and written back to HBM only when a selector moves to another set; dot
+//    products and SGD use all 512 lanes (integer sums: exact under any association).
+// The 55 KB state block and the hot read-only tables (21 KB) live in the shared memory of both CTAs for the launch, the
+// 87 KB weight cache and the ring in the mixer CTA's; the ~10 GB of model memory stays in HBM. Each CTA writes back the
+// fields of the state block it owns (p8_leave).
 // PAQ8 is a producer like FXCM: it depends on the coded bytes only and writes 1591 codes per bit into the `ext` scratch.
 #pragma once
+#include <cooperative_groups.h>
 #include "paq8_top.h"
 #include "state.h"
 
 namespace cmixb200 {
 
-enum { P8_SEEN = 4096 };
+enum { P8_SEEN = 4096, P8_RING = 4 };
 
-// -DP8_PROF: lane 0 accumulates the cycles between phase boundaries (byte-boundary bits and the others apart)
+// -DP8_PROF: lane 0 of each CTA accumulates the cycles between phase boundaries (byte-boundary bits and the others apart):
+// slots 0-11 the model CTA (10: waiting for a free ring slot), 16-19 the mixer CTA (16: waiting for a full one), 24+ per-warp
+// times of the model phases
 #ifdef P8_PROF
 __device__ unsigned long long g_p8_prof[2][96];
 #define P8_T(k) do { if (tid == 0) { const long long now_ = clock64(); atomicAdd(&g_p8_prof[sh.prof_row][k], (unsigned long long)(now_ - sh.prof_t)); sh.prof_t = now_; } } while (0)
@@ -44,16 +54,28 @@ __device__ unsigned long long g_p8_prof[2][96];
 #define P8_M(slot) do { } while (0)
 #define P8_C(slot, n) do { } while (0)
 #endif
-enum { P8_THREADS = 512, P8_WARPS = 16, P8_MAP_THREADS = 384, P8_MAP_WARPS = 12, P8_SGD_THREADS = 128, P8_N_CM = 16, P8_N_CM2 = 3, P8_CM_LANES = 210, P8_CM2_LANES = 63, P8_N_UNITS = 53,
+enum { P8_THREADS = 512, P8_WARPS = 16, P8_MAP_THREADS = 384, P8_MAP_WARPS = 12, P8_N_CM = 16, P8_N_CM2 = 3, P8_CM_LANES = 210, P8_CM2_LANES = 63, P8_N_UNITS = 53,
        P8_CM2_TID0 = 224, P8_TID_PIC = 287, P8_TID_MATCH = 288, P8_TID_W10 = 320, P8_TID_W11 = 352 };
+
+// One bit handed from the model CTA to the mixer CTA: what the models produced and the context the SSE stage reads.
+struct P8Slot {
+  alignas(16) short tx[p8::N_IN];    // mixer inputs [0, nx), zero-padded to a multiple of 8
+  alignas(16) u16 codes[p8::N_IN];   // their exported codes [0, n2)
+  int cxt[p8::N_SETS];               // the selected weight sets; set 26 is the mixer CTA's (it depends on its last prediction)
+  int n2, nx, ncxt, base;
+  int c0, bpos, blpos, st_type; u32 c4, st_match_length;
+  u8 c1, st_match_expected, st_text_first, st_text_mask;
+};
 
 struct P8Shared {
   p8::State S;
-  alignas(16) short wc[p8::N_SETS][p8::N_IN];   // the weight sets of the pending prediction (slot i holds set wc_set[i])
   alignas(16) unsigned char tab[p8::TABLES_HOT_BYTES];
-  alignas(16) short tx_old[p8::N_IN];           // the inputs of the previous bit: the SGD warps train while the map warps write new ones
+  alignas(8) unsigned long long full[P8_RING];    // in the mixer CTA: slot i holds a bit (one arrive per model warp)
+  unsigned long long empty[P8_RING];              // in the model CTA: the mixer CTA is done with slot i
+  // mixer CTA
   int wc_set[p8::N_SETS];
-  int sgd_err[p8::N_SETS], sgd_nx, sgd_ncxt;
+  int dot[p8::N_SETS];
+  // model CTA
   int unit_off[P8_N_UNITS + 1];
   // pass-1 results of the 7-slot maps
   short ns[P8_CM_LANES];
@@ -61,7 +83,6 @@ struct P8Shared {
   u32 ids2[P8_CM2_LANES][5];
   int clash[P8_N_CM], clash2[P8_N_CM2];
   int order, res2[P8_N_CM2];
-  int dot[p8::N_SETS];
   u32 snap_spaces, snap_words, snap_frstchar, snap_spafdo;
   int dmc_st[10];
   u32 flag_mask[8];            // ballot of "this context draws" per warp of map lanes
@@ -72,6 +93,10 @@ struct P8Shared {
   union {
     unsigned long long seen[P8_SEEN];   // open-addressing set of (map, bucket) pairs touched this bit
     struct { double ch[3][32 * 33]; double pb[3][32]; } ols;   // Cholesky factor rows (padded) and a product buffer; byte boundaries only
+    struct {                                                    // the mixer CTA
+      alignas(16) short wc[p8::N_SETS][p8::N_IN];   // the weight sets of the pending prediction (slot i holds set wc_set[i])
+      P8Slot ring[P8_RING];
+    } mx;
   } u;
 #ifdef P8_PROF
   long long prof_t; int prof_row;
@@ -404,8 +429,8 @@ __device__ __noinline__ void p8_apply_small(P8Shared& sh, int tid, int y, int bp
   }
 }
 
-// The SSE stage (paq8_top.h sse_stage) on one warp: the APMs of a level side by side.
-__device__ void p8_sse_warp(P8Shared& sh, int pr0, int lane) {
+// The SSE stage (paq8_top.h sse_stage) on one warp: the APMs of a level side by side. c1 = buf(S, 1) of the bit.
+__device__ void p8_sse_warp(P8Shared& sh, int pr0, int c1, int lane) {
   using namespace p8;
   State& S = sh.S;
   const p8::Tables& T = *S.T;
@@ -435,7 +460,7 @@ __device__ void p8_sse_warp(P8Shared& sh, int pr0, int lane) {
       q = apm1_p(T, S.text_apm1[lane], y, lane == 0 ? pr0b : pr, cx, lane == 0 ? 7 : 6);
     }
   } else {
-    const u16 ctx1 = (u16)(c0 | buf(S, 1) << 8);
+    const u16 ctx1 = (u16)(c0 | c1 << 8);
     const u16 ctx2 = (u16)(c0 ^ finalize64(hash((u64)(c4 & 0xffff)), 16));
     const u16 ctx3 = (u16)(c0 ^ finalize64(hash((u64)(c4 & 0xffffff)), 16));
     if (lane < 4) {
@@ -445,7 +470,7 @@ __device__ void p8_sse_warp(P8Shared& sh, int pr0, int lane) {
     pr = __shfl_sync(full, p, 0); pr1 = __shfl_sync(full, p, 1); pr2 = __shfl_sync(full, p, 2); pr3 = __shfl_sync(full, p, 3);
     pr0b = (pr0 + pr1 + pr2 + pr3 + 2) >> 2;
     if (lane < 3) {
-      const int cx = lane == 0 ? ((S.st_match_expected << 8) | buf(S, 1)) : lane == 1 ? (int)ctx2 : (int)ctx3;
+      const int cx = lane == 0 ? ((S.st_match_expected << 8) | c1) : lane == 1 ? (int)ctx2 : (int)ctx3;
       q = apm1_p(T, S.generic_apm1[4 + lane], y, pr, cx);
     }
   }
@@ -484,31 +509,52 @@ __device__ __forceinline__ void p8_signal_selects() { asm volatile("bar.arrive 2
 __device__ __forceinline__ void p8_await_selects() { asm volatile("bar.sync 2, 416;" ::: "memory"); }
 __device__ __forceinline__ void p8_sync_maps() { asm volatile("bar.sync 1, 384;" ::: "memory"); static_assert(P8_MAP_THREADS == 384, "named barrier width"); }
 
-// Mixer::update for the 28 cached weight sets selected for the previous bit, by the four SGD warps (tid 0..127 of them)
-__device__ __forceinline__ void p8_sgd(P8Shared& sh, int t) {
+// The ring's mbarriers. An arrive on the other CTA's barrier releases at cluster scope what the arriving thread wrote or
+// read before it; a wait acquires it.
+__device__ __forceinline__ u32 p8_smem(const void* p) { return (u32)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void p8_mbar_init(unsigned long long* b, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(p8_smem(b)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void p8_mbar_arrive_remote(unsigned long long* b, int rank) {
+  u32 r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(p8_smem(b)), "r"(rank));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(r) : "memory");
+}
+__device__ __forceinline__ void p8_mbar_wait(unsigned long long* b, u32 parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "P8W: mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
+      "@!p bra P8W;\n\t}" ::"r"(p8_smem(b)), "r"(parity) : "memory");
+}
+
+// Mixer::update for the 28 cached weight sets selected for the previous bit, on its inputs tx (all lanes of the mixer CTA)
+__device__ __forceinline__ void p8_sgd(P8Shared& sh, const short* tx, int y, int tid) {
   using namespace p8;
-  const int n8 = sh.sgd_nx >> 3, total = sh.sgd_ncxt * n8;
+  const Mixer& m = sh.S.m;
+  const int n8 = m.nx >> 3, total = m.ncxt * n8;
   if (n8 == 0) return;
-  int i = t / n8, q = t - i * n8;
-  for (int idx = t; idx < total; idx += P8_SGD_THREADS) {
-    const int err = sh.sgd_err[i];
+  int i = tid / n8, q = tid - i * n8;
+  for (int idx = tid; idx < total; idx += P8_THREADS) {
+    const int err = ((y << 12) - m.pr[i]) * 7;
     if (err) {
-      uint4* wp = reinterpret_cast<uint4*>(&sh.wc[i][q * 8]);
+      uint4* wp = reinterpret_cast<uint4*>(&sh.u.mx.wc[i][q * 8]);
       uint4 wv = *wp;
-      const uint4 xv = *reinterpret_cast<const uint4*>(&sh.tx_old[q * 8]);
+      const uint4 xv = *reinterpret_cast<const uint4*>(&tx[q * 8]);
       short* w = reinterpret_cast<short*>(&wv);
       const short* x = reinterpret_cast<const short*>(&xv);
 #pragma unroll
       for (int e = 0; e < 8; ++e) w[e] = train_one(x[e], w[e], err);
       *wp = wv;
     }
-    q += P8_SGD_THREADS;
+    q += P8_THREADS;
     while (q >= n8) { q -= n8; ++i; }
   }
 }
 
-// One bit: PAQ8::Perceive(y). All P8_THREADS lanes call it: warps 0-11 evaluate the models, warps 12-15 train the mixer beside them.
-__device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false) {   // nb: the bit position after this bit, (S.bpos + 1) & 7; fresh: shared memory holds nothing from the previous bit
+// The model CTA's part of bit t of a launch: PAQ8::Perceive(y) up to the mixer's inputs and selectors, handed to slot t % P8_RING
+// of the mixer CTA's ring (`ring`: that array in the mixer CTA). All P8_THREADS lanes call it: warps 0-11 evaluate the models,
+// warp 12 computes ModelStats and 19 selector sets beside them.
+__device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, int tid, bool fresh = false) {   // nb: the bit position after this bit, (S.bpos + 1) & 7; fresh: shared memory holds nothing from the previous bit
   using namespace p8;
   State& S = sh.S;
   const p8::Tables& T = *S.T;
@@ -516,9 +562,8 @@ __device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false)
 #ifdef P8_PROF
   if (tid == 0) { sh.prof_t = clock64(); sh.prof_row = (S.bpos == 7) ? 0 : 1; }   // bpos before bit_begin: 7 -> this bit starts a byte
 #endif
-  // ---- phase 0: bookkeeping; the previous bit's inputs and errors move aside for the SGD warps
+  // ---- phase 0: bookkeeping (bit_begin's st_misses line works on a stale S.pr here: st_misses belongs to the mixer CTA)
   if (tid == 0) {
-    sh.sgd_nx = S.m.nx; sh.sgd_ncxt = S.m.ncxt;
     bit_begin(S, y);
     if (S.bpos == 0) block_parse(S);
     sh.snap_spaces = S.spaces; sh.snap_words = S.words; sh.snap_frstchar = S.frstchar; sh.snap_spafdo = S.spafdo;
@@ -527,8 +572,6 @@ __device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false)
   if (tid >= 64 && tid < 64 + P8_N_CM2) { sh.clash2[tid - 64] = 0; sh.res2[tid - 64] = 0; }
   if (tid == 67) { sh.any_clash = 0; sh.rnd_prev_i = S.rnd.i; }
   if (tid >= 320 && tid < 384) sh.rnd_prev[tid - 320] = S.rnd.table[tid - 320];
-  if (tid >= 96 && tid < 96 + N_SETS) sh.sgd_err[tid - 96] = ((y << 12) - S.m.pr[tid - 96]) * 7;
-  if (tid >= 128 && tid < 128 + N_IN / 8) reinterpret_cast<uint4*>(sh.tx_old)[tid - 128] = reinterpret_cast<const uint4*>(S.m.tx)[tid - 128];
   if (tid >= P8_CM2_TID0 && tid < P8_CM2_TID0 + P8_N_CM2) cm2_begin(p8_cm2(S, tid - P8_CM2_TID0), y, nb);
   if (warp == P8_WARPS - 1 && (nb <= 1 || fresh)) {      // mixer-input offsets of the units (they change on the first two bits of a byte only)
     const unsigned full = 0xffffffffu;
@@ -550,7 +593,6 @@ __device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false)
   const int bpos = S.bpos, c0 = S.c0;
   const bool byte_start = bpos == 0;
   if (tid >= P8_MAP_THREADS) {
-    p8_sgd(sh, tid - P8_MAP_THREADS);
     if (warp == P8_MAP_WARPS) {            // ModelStats and the 19 selector sets that do not wait for the order-N map
       p8_await_selects();
       if (lane == 0) {
@@ -680,29 +722,85 @@ __device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false)
         for (int k = 0; k < P8_N_CM; ++k) if (!sh.clash[k]) p8_cm(S, k).cn = 0;
         for (int k = 0; k < P8_N_CM2; ++k) p8_cm2(S, k).index = 0;
       }
-      main_select_fixed(S, sh.res2[0]);      // sets 19..27; the first SGD warp writes 0..18 (and the count) beside this
+      main_select_fixed(S, sh.res2[0]);      // sets 19..27; warp 12 writes 0..18 (and the count) beside this
       Mixer& m = S.m;
       m.nx = sh.unit_off[P8_N_UNITS];
       m.n2 = m.nx;
       while (m.nx & 7) m.tx[m.nx++] = 0;
     }
   }
-  __syncthreads();     // the SGD warps join
+  __syncthreads();     // warp 12 joins
   P8_T(9);
-  // ---- final-mixer SGD (32 weights); the 28 dot products over the cached sets (a selector that moved: write back, load)
+  // ---- hand the bit over. Only warp 0 reads the scalars: its lane 0 is the one that changes them at the next bit's start,
+  // the other warps' data (inputs, codes) changes only after the next bit's first barrier.
+  const int slot = (int)(t % P8_RING);
+  if (t >= P8_RING) p8_mbar_wait(&sh.empty[slot], (t / P8_RING - 1) & 1);
+  P8_T(10);
   {
-    Mixer& m = S.m;
-    if (warp == P8_WARPS - 1) {
-      const int err = ((y << 12) - m.pr2) * 7;
-      if (err && lane < m.nx2) m.w2[lane] = train_one(m.tx2[lane], m.w2[lane], err);
+    const Mixer& m = S.m;
+    P8Slot& d = ring[slot];
+    if (warp == 0) {
+      if (lane < N_SETS) d.cxt[lane] = m.cxt[lane];
+      if (lane == 0) {
+        d.n2 = m.n2; d.nx = m.nx; d.ncxt = m.ncxt; d.base = m.base;
+        d.c0 = S.c0; d.bpos = S.bpos; d.blpos = S.blpos; d.st_type = S.st_type; d.c4 = S.c4; d.st_match_length = S.st_match_length;
+        d.c1 = (u8)buf(S, 1); d.st_match_expected = S.st_match_expected; d.st_text_first = S.st_text_first; d.st_text_mask = S.st_text_mask;
+      }
     }
-    if (warp == P8_WARPS - 2 && lane < m.ncxt) {        // two selectors on one weight set would need the reference's sequential SGD
+    for (int q = tid; q < m.nx / 8; q += P8_THREADS) reinterpret_cast<uint4*>(d.tx)[q] = reinterpret_cast<const uint4*>(m.tx)[q];
+    for (int q = tid; q < (m.n2 + 1) / 2; q += P8_THREADS) reinterpret_cast<u32*>(d.codes)[q] = reinterpret_cast<const u32*>(S.codes)[q];
+    __syncwarp();
+    if (lane == 0) p8_mbar_arrive_remote(&sh.full[slot], 1);
+  }
+  P8_T(11);
+}
+static_assert(offsetof(p8::State, codes) % 4 == 0 && p8::N_IN % 2 == 0, "codes are handed over in 4-byte words");
+
+// The mixer CTA's part of bit t of a launch (y, and nb as in p8_model_bit): the SGD of the sets picked for bit t-1 on its
+// inputs (tx_prev) and of the final mixer, which need only the bit and so run beside the model CTA's work on it; then, from
+// ring slot t % P8_RING, the 28 dot products, squash, the final mixer and the SSE stage. S.codes then holds the 1591 codes
+// after the bit.
+__device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_prev, int tid) {
+  using namespace p8;
+  State& S = sh.S;
+  const p8::Tables& T = *S.T;
+  Mixer& m = S.m;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int slot = (int)(t % P8_RING);
+  const P8Slot& in = sh.u.mx.ring[slot];
+#ifdef P8_PROF
+  if (tid == 0) { sh.prof_t = clock64(); sh.prof_row = nb == 0 ? 0 : 1; }
+#endif
+  // ---- SGD of the previous bit's sets and of the final mixer
+  p8_sgd(sh, tx_prev, y, tid);
+  if (warp == P8_WARPS - 1) {
+    const int err = ((y << 12) - m.pr2) * 7;
+    if (err && lane < m.nx2) m.w2[lane] = train_one(m.tx2[lane], m.w2[lane], err);
+  }
+  P8_T(17);
+  // ---- the bit's inputs and selectors (set 26 from this CTA's last prediction)
+  p8_mbar_wait(&sh.full[slot], (t / P8_RING) & 1);
+  P8_T(16);
+  if (tid < N_SETS) m.cxt[tid] = tid == MAIN_SET_FIRST + 7 ? MAIN_SET_PR + S.last_prediction / 16 : in.cxt[tid];
+  __syncthreads();
+  if (tid == 0) {
+    if (t > 0) p8_mbar_arrive_remote(&sh.empty[(t - 1) % P8_RING], 0);   // tx_prev was slot t-1's
+    S.st_misses += S.st_misses + (u64)((S.pr >> 11) != y);               // bit_begin's line, on this CTA's prediction
+    S.y = y; S.c0 = in.c0; S.bpos = in.bpos; S.blpos = in.blpos; S.c4 = in.c4; S.st_type = in.st_type;
+    S.st_match_length = in.st_match_length; S.st_match_expected = in.st_match_expected;
+    S.st_text_first = in.st_text_first; S.st_text_mask = in.st_text_mask;
+    m.n2 = in.n2; m.nx = in.nx; m.ncxt = in.ncxt; m.base = in.base;
+  }
+  // ---- the 28 dot products over the cached sets (a selector that moved: write back, load)
+  {
+    for (int q = tid; q < (in.n2 + 1) / 2; q += P8_THREADS) reinterpret_cast<u32*>(S.codes)[q] = reinterpret_cast<const u32*>(in.codes)[q];
+    if (warp == P8_WARPS - 2 && lane < in.ncxt) {        // two selectors on one weight set would need the reference's sequential SGD
       bool dup = false;
       for (int j = 0; j < lane; ++j) dup = dup || m.cxt[j] == m.cxt[lane];
       if (dup) S.error |= ERR_MIXER_ALIAS;
     }
-    for (int i = warp; i < m.ncxt; i += P8_WARPS) {
-      short* row = sh.wc[i];
+    for (int i = warp; i < in.ncxt; i += P8_WARPS) {
+      short* row = sh.u.mx.wc[i];
       const int set = m.cxt[i], old = sh.wc_set[i];
       if (old != set) {
         if (old >= 0) p8_row_store(m.w + (size_t)old * N_IN, row, lane);
@@ -711,10 +809,10 @@ __device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false)
         if (lane == 0) sh.wc_set[i] = set;
       }
       int acc = 0;
-      const int n8 = m.nx >> 3;
+      const int n8 = in.nx >> 3;
       for (int q = lane; q < n8; q += 32) {
         const uint4 wv = *reinterpret_cast<const uint4*>(row + q * 8);
-        const uint4 xv = *reinterpret_cast<const uint4*>(m.tx + q * 8);
+        const uint4 xv = *reinterpret_cast<const uint4*>(in.tx + q * 8);
         const short* w = reinterpret_cast<const short*>(&wv);
         const short* x = reinterpret_cast<const short*>(&xv);
 #pragma unroll
@@ -725,10 +823,9 @@ __device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false)
     }
   }
   __syncthreads();
-  P8_T(10);
+  P8_T(18);
   // ---- squash, final mixer, SSE stage (one warp)
   if (warp == 0) {
-    Mixer& m = S.m;
     const int base = m.n2, n = m.ncxt, nx2 = (n + 7) & ~7;
     int x = 0;
     if (lane < n) {
@@ -744,71 +841,114 @@ __device__ void p8_bit(P8Shared& sh, int y, int nb, int tid, bool fresh = false)
     const int pr2 = squash(T, z >> 9);
     if (lane == 0) { m.nx2 = nx2; m.pr2 = pr2; }
     __syncwarp();
-    p8_sse_warp(sh, pr2, lane);
+    p8_sse_warp(sh, pr2, in.c1, lane);
   }
   __syncthreads();
-  P8_T(11);
+  P8_T(19);
 }
 
-// state block, hot tables and the pending weight sets into shared memory
-__device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g, int tid) {
+// Both CTAs: state block and hot tables into shared memory, the ring's barriers; the mixer CTA: the pending weight sets.
+__device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g, int tid, int rank) {
   p8_copy_words(&sh.S, g, sizeof(p8::State), tid);
   __syncthreads();
   const p8::Tables* gT = sh.S.T;
   p8_copy_words(sh.tab, gT, p8::TABLES_HOT_BYTES, tid);
   if (tid < p8::N_SETS) sh.wc_set[tid] = -1;
+  if (tid == 0) {
+    for (int i = 0; i < P8_RING; ++i) {
+      if (rank == 0) p8_mbar_init(&sh.empty[i], 1);
+      else p8_mbar_init(&sh.full[i], P8_WARPS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
   __syncthreads();
   if (tid == 0) sh.S.T = reinterpret_cast<const p8::Tables*>(sh.tab);
   const int warp = tid >> 5, lane = tid & 31;
-  for (int i = warp; i < sh.S.m.ncxt; i += P8_WARPS) {
-    p8_row_load(sh.wc[i], sh.S.m.w + (size_t)sh.S.m.cxt[i] * p8::N_IN, lane);
-    if (lane == 0) sh.wc_set[i] = sh.S.m.cxt[i];
+  if (rank == 1) {
+    for (int i = warp; i < sh.S.m.ncxt; i += P8_WARPS) {
+      p8_row_load(sh.u.mx.wc[i], sh.S.m.w + (size_t)sh.S.m.cxt[i] * p8::N_IN, lane);
+      if (lane == 0) sh.wc_set[i] = sh.S.m.cxt[i];
+    }
   }
-  __syncthreads();
+  cooperative_groups::this_cluster().sync();   // the barriers exist before the other CTA arrives on them
   return gT;
 }
-__device__ __forceinline__ void p8_leave(P8Shared& sh, p8::State* g, const p8::Tables* gT, int tid) {
-  __syncthreads();
+// Each CTA writes back the fields it owns: the mixer CTA `m`, the APMs and `codes` (with the inputs of the last bit it
+// took, `last` = its ring slot, or none), the model CTA everything before `m` and `error`, after taking `pr`,
+// `last_prediction` and `st_misses` from the mixer CTA and OR-ing its error bits into its own.
+__device__ __forceinline__ void p8_leave(P8Shared& sh, p8::State* g, const p8::Tables* gT, int tid, int rank, int last) {
+  using namespace p8;
+  cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
   const int warp = tid >> 5, lane = tid & 31;
-  for (int i = warp; i < p8::N_SETS; i += P8_WARPS)
-    if (sh.wc_set[i] >= 0) p8_row_store(sh.S.m.w + (size_t)sh.wc_set[i] * p8::N_IN, sh.wc[i], lane);
-  if (tid == 0) sh.S.T = gT;
-  __syncthreads();
-  p8_copy_words(g, &sh.S, sizeof(p8::State), tid);
+  if (rank == 1) {
+    for (int i = warp; i < N_SETS; i += P8_WARPS)
+      if (sh.wc_set[i] >= 0) p8_row_store(sh.S.m.w + (size_t)sh.wc_set[i] * N_IN, sh.u.mx.wc[i], lane);
+    if (last >= 0) for (int q = tid; q < sh.S.m.nx / 8; q += P8_THREADS) reinterpret_cast<uint4*>(sh.S.m.tx)[q] = reinterpret_cast<const uint4*>(sh.u.mx.ring[last].tx)[q];
+  }
+  cluster.sync();
+  if (rank == 0 && tid == 0) {
+    const State& X = cluster.map_shared_rank(&sh, 1)->S;
+    sh.S.pr = X.pr; sh.S.last_prediction = X.last_prediction; sh.S.st_misses = X.st_misses;
+    sh.S.error |= X.error;
+    sh.S.T = gT;
+  }
+  cluster.sync();   // the mixer CTA's shared memory stays until the model CTA has read it
+  const size_t m0 = offsetof(State, m), e0 = offsetof(State, error);
+  static_assert(offsetof(State, m) % 4 == 0 && offsetof(State, error) % 4 == 0, "state block is copied word by word");
+  if (rank == 0) {
+    p8_copy_words(g, &sh.S, m0, tid);
+    p8_copy_words((char*)g + e0, (const char*)&sh.S + e0, sizeof(State) - e0, tid);
+  } else {
+    p8_copy_words((char*)g + m0, (const char*)&sh.S + m0, e0 - m0, tid);
+  }
 }
 
-// Bulk: CTA b serves stream b of the launch group: writes ext[t][431..2021] for every bit t of the sub-chunk.
-__global__ void __launch_bounds__(P8_THREADS, 1) paq8_kernel(const ChunkArgs* __restrict__ args_all) {
+// Bulk: cluster b (CTAs 2b, 2b+1) serves stream b of the launch group: writes ext[t][431..2021] for every bit t of the sub-chunk.
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P8_THREADS, 1) paq8_kernel(const ChunkArgs* __restrict__ args_all) {
   extern __shared__ __align__(16) unsigned char p8_raw[];
   P8Shared& sh = *reinterpret_cast<P8Shared*>(p8_raw);
-  const ChunkArgs a = args_all[blockIdx.x];
+  const ChunkArgs a = args_all[blockIdx.x >> 1];
   if (a.paq8 == nullptr) return;
   const int tid = threadIdx.x;
+  const int rank = (int)cooperative_groups::this_cluster().block_rank();
   p8::State* g = (p8::State*)a.paq8;
-  const p8::Tables* gT = p8_enter(sh, g, tid);
+  const p8::Tables* gT = p8_enter(sh, g, tid, rank);
   const u32 n_bits = a.n_bytes * 8;
-  for (u32 t = 0; t < n_bits; ++t) {
-    if (!a.pretrain) {
-      u16* out = a.ext_gen + (size_t)t * N_EXT + 431;
-      for (int k = tid; k < p8::N_OUT; k += P8_THREADS) out[k] = sh.S.codes[k];
+  if (rank == 0) {
+    P8Slot* ring = cooperative_groups::this_cluster().map_shared_rank(&sh, 1)->u.mx.ring;
+    for (u32 t = 0; t < n_bits; ++t) {
+      const int y = (a.bytes[t >> 3] >> (7 - (t & 7))) & 1;
+      p8_model_bit(sh, ring, t, y, (int)((t + 1) & 7), tid);
     }
-    const int y = (a.bytes[t >> 3] >> (7 - (t & 7))) & 1;
-    p8_bit(sh, y, (int)((t + 1) & 7), tid);
+  } else {
+    for (u32 t = 0; t < n_bits; ++t) {
+      if (!a.pretrain) {
+        u16* out = a.ext_gen + (size_t)t * N_EXT + 431;
+        for (int k = tid; k < p8::N_OUT; k += P8_THREADS) out[k] = sh.S.codes[k];
+      }
+      const int y = (a.bytes[t >> 3] >> (7 - (t & 7))) & 1;
+      p8_mix_bit(sh, t, y, (int)((t + 1) & 7), t == 0 ? sh.S.m.tx : sh.u.mx.ring[(t - 1) % P8_RING].tx, tid);
+    }
   }
-  p8_leave(sh, g, gT, tid);
+  p8_leave(sh, g, gT, tid, rank, n_bits ? (int)((n_bits - 1) % P8_RING) : -1);
 }
 
-// Lock-step: one bit per launch; the codes for the next Predict() land in ext_bit[431..2021].
-__global__ void __launch_bounds__(P8_THREADS, 1) paq8_bit_kernel(p8::State* g, int y, u16* ext_bit, const u32* dbit) {
+// Lock-step: one bit per launch, a one-slot handover; the codes for the next Predict() land in ext_bit[431..2021].
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P8_THREADS, 1) paq8_bit_kernel(p8::State* g, int y, u16* ext_bit, const u32* dbit) {
   if (dbit) y = (int)dbit[0];
   extern __shared__ __align__(16) unsigned char p8_raw[];
   P8Shared& sh = *reinterpret_cast<P8Shared*>(p8_raw);
   const int tid = threadIdx.x;
-  const int nb = (g->bpos + 1) & 7;       // read from HBM: the shared copy is being updated by lane 0 inside p8_bit
-  const p8::Tables* gT = p8_enter(sh, g, tid);
-  p8_bit(sh, y, nb, tid, true);
-  if (ext_bit) for (int k = tid; k < p8::N_OUT; k += P8_THREADS) ext_bit[431 + k] = sh.S.codes[k];
-  p8_leave(sh, g, gT, tid);
+  const int rank = (int)cooperative_groups::this_cluster().block_rank();
+  const int nb = (g->bpos + 1) & 7;       // read from HBM: the shared copy is being updated by lane 0 inside p8_model_bit
+  const p8::Tables* gT = p8_enter(sh, g, tid, rank);
+  if (rank == 0) {
+    p8_model_bit(sh, cooperative_groups::this_cluster().map_shared_rank(&sh, 1)->u.mx.ring, 0, y, nb, tid, true);
+  } else {
+    p8_mix_bit(sh, 0, y, nb, sh.S.m.tx, tid);
+    if (ext_bit) for (int k = tid; k < p8::N_OUT; k += P8_THREADS) ext_bit[431 + k] = sh.S.codes[k];
+  }
+  p8_leave(sh, g, gT, tid, rank, 0);
 }
 
 }  // namespace cmixb200

@@ -9,11 +9,11 @@ cudaError_t paq8_configure() {
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(paq8_bit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(P8Shared));
 }
-void paq8_launch_chunk(const ChunkArgs* d_args, int n_streams, cudaStream_t s) {
-  paq8_kernel<<<n_streams, P8_THREADS, sizeof(P8Shared), s>>>(d_args);
+void paq8_launch_chunk(const ChunkArgs* d_args, int n_streams, cudaStream_t s) {   // a cluster of two CTAs per stream
+  paq8_kernel<<<2 * n_streams, P8_THREADS, sizeof(P8Shared), s>>>(d_args);
 }
 void paq8_launch_bit(p8::State* g, int y, u16* ext_bit, cudaStream_t s, const u32* dbit) {
-  paq8_bit_kernel<<<1, P8_THREADS, sizeof(P8Shared), s>>>(g, y, ext_bit, dbit);
+  paq8_bit_kernel<<<2, P8_THREADS, sizeof(P8Shared), s>>>(g, y, ext_bit, dbit);
 }
 
 }  // namespace cmixb200

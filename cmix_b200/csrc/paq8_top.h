@@ -827,8 +827,9 @@ P8_HD inline void main_select(State& S, int order) {   // the nine selector sets
 
 // The same nine sets written at their fixed places: the 19 sets before them always cover MAIN_SET_BASE weight sets, so a lane can
 // compute these while another one is still producing the first 19 (paq8.cuh).
-enum { MAIN_SET_FIRST = 19, MAIN_SET_BASE = 66656 };
-static_assert(MAIN_SET_BASE + 64 + 4 * 1536 + 2 * 2048 + 2 * 256 == N_WSETS && MAIN_SET_FIRST + 9 == N_SETS, "selector layout");
+// MAIN_SET_PR: the first weight set of selector MAIN_SET_FIRST + 7, the one indexed by the last prediction.
+enum { MAIN_SET_FIRST = 19, MAIN_SET_BASE = 66656, MAIN_SET_PR = MAIN_SET_BASE + 64 + 4 * 1536 + 2 * 2048 };
+static_assert(MAIN_SET_PR + 2 * 256 == N_WSETS && MAIN_SET_FIRST + 9 == N_SETS, "selector layout");
 P8_HD inline void main_select_fixed(State& S, int order) {
   Mixer& m = S.m;
   const int bpos = S.bpos, c0 = S.c0;

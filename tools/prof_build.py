@@ -67,7 +67,12 @@ def run(n_bytes):
         for k in range(rows):
             if a[0, k] or a[1, k]:
                 print("  phase %2d  %9.0f | %9.0f" % (k, a[0, k] / n_bytes, a[1, k] / (7 * n_bytes)))
-        print("  total     %9.0f | %9.0f   -> %.1f us/bit average" % (a[0, :24].sum() / n_bytes, a[1, :24].sum() / (7 * n_bytes), a[:, :24].sum() / (8 * n_bytes) / sm_mhz))
+        # PAQ8 runs on two CTAs: the model CTA counts in slots 0-15 (10: waiting for a free ring slot), the mixer CTA in
+        # 16-23 (16: waiting for a full slot); each CTA's total is its time per bit, less the mixer CTA's code-row writes
+        parts = (("model CTA", 0, 16), ("mixer CTA", 16, 24)) if name == "paq8" else (("total", 0, 24),)
+        for label, lo, hi in parts:
+            print("  %-9s %9.0f | %9.0f   -> %.1f us/bit average" % (label, a[0, lo:hi].sum() / n_bytes, a[1, lo:hi].sum() / (7 * n_bytes),
+                                                                    a[:, lo:hi].sum() / (8 * n_bytes) / sm_mhz))
     P.close()
 
 
