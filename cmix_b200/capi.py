@@ -75,8 +75,6 @@ def load_library():
     lib.cmixb200_kernel_launches.restype = c.c_ulonglong
     lib.cmixb200_time_mix_kernel.argtypes = [vp, c.c_int]
     lib.cmixb200_time_mix_kernel.restype = None
-    lib.cmixb200_mix_kernel_ms.argtypes = [vp, c.POINTER(c.c_ulonglong)]
-    lib.cmixb200_mix_kernel_ms.restype = c.c_double
     lib.cmixb200_kernel_ms.argtypes = [vp, c.c_int, c.POINTER(c.c_ulonglong)]
     lib.cmixb200_kernel_ms.restype = c.c_double
     lib.cmixb200_mix_stream.argtypes = [vp]
@@ -199,11 +197,6 @@ class Predictor:
 
     def time_mix_kernel(self, enable=True):
         self._lib.cmixb200_time_mix_kernel(self._h, 1 if enable else 0)
-
-    def mix_kernel_ms(self):
-        n = ctypes.c_ulonglong(0)
-        ms = self._lib.cmixb200_mix_kernel_ms(self._h, ctypes.byref(n))
-        return float(ms), int(n.value)
 
     def kernel_ms(self, which):
         """(total ms, launches) of one bulk kernel since time_mix_kernel(True): 0 mix, 1 small, 2 lstm, 3 ppmd, 4 fxcm, 5 paq8."""

@@ -97,11 +97,10 @@ int cmixb200_pretrain_bytes(cmixb200_predictor*, const uint8_t* bytes, size_t n_
 const char* cmixb200_last_error(void);
 /* kernels launched by this predictor so far (bench.py's gpu_launches). */
 unsigned long long cmixb200_kernel_launches(const cmixb200_predictor*);
-/* CUDA-event timing of the mixer kernel on the stream it is launched on (bench.py's roofline):
- * enable, run bulk calls, then read the accumulated milliseconds and launch count. */
+/* CUDA-event timing of every bulk kernel on the stream it is launched on (bench.py's roofline):
+ * enable, run bulk calls, then read the accumulated milliseconds and launch count of one kernel:
+ * which = 0 mixer, 1 small models, 2 LSTM, 3 PPMD, 4 FXCM, 5 PAQ8 (each on its own CUDA stream). */
 void cmixb200_time_mix_kernel(cmixb200_predictor*, int enable);
-double cmixb200_mix_kernel_ms(const cmixb200_predictor*, unsigned long long* n_launches);
-/* the same for every bulk kernel: which = 0 mixer, 1 small models, 2 LSTM, 3 PPMD, 4 FXCM, 5 PAQ8 (each on its own CUDA stream) */
 double cmixb200_kernel_ms(const cmixb200_predictor*, int which, unsigned long long* n_launches);
 /* the cudaStream_t the mixer kernel runs on (for CUDA-event timing in bench.py). */
 void* cmixb200_mix_stream(cmixb200_predictor*);

@@ -187,6 +187,31 @@ def test_decode_after_pretraining(cm, port, dict_path, pre):
 
 
 @pytest.mark.timeout(900)
+def test_decode_then_lock_step(cm):
+    """Lock-step after the decoder: the first Predict() is ordered behind the decoder's last graph and takes the codes its
+    FXCM and PAQ8 bit kernels left in d_ext_bit; a bulk call follows."""
+    g = _load("full_text")
+    s, p = g["stream"], g["p"]
+    n, m = 256, 288
+    sched = "full_text: coded/decoded [0,%d), lock-step [%d,%d), bulk [%d,1024)" % (n, n, m, m)
+    enc = cm.Predictor(g["vocab"])
+    try:
+        enc.coder_begin(2 * n + 64)
+        _expect(sched + ", encoder bulk", enc.code_bytes(s[:n]), p[:n * 8])
+        archive = enc.coder_finish()
+    finally:
+        enc.close()
+    dec = cm.Predictor(g["vocab"])
+    try:
+        out = dec.decode_bytes(archive, n)
+        assert out.tobytes() == s[:n].tobytes(), "%s, decoder: %s" % (sched, _first_bad_byte(out, s[:n]))
+        _lock_step(dec, g, n * 8, m * 8, sched)
+        _expect(sched + ", bulk", dec.code_bytes(s[m:1024]), p[m * 8:1024 * 8], m * 8)
+    finally:
+        dec.close()
+
+
+@pytest.mark.timeout(900)
 def test_bulk_split_schedule(cm):
     """Bulk calls of 1, 16, 17, 129, 257, 4097 and 1627 bytes: n <= 16, the halving tail, the geometric head and full
     sub-chunks of RunPipelined, RunPieces' 2048-byte pieces and code_bytes' 4096-byte host staging; together = one call."""
