@@ -35,8 +35,8 @@
 #include "paq8_host.h"
 #include "producers.h"
 #include "lstm.cuh"
-#include "mixer.cuh"
-#include "mixer_v3.cuh"
+#include "mixer_lock.cuh"
+#include "mixer_bulk.cuh"
 #include "ppmd.cuh"
 #include "small_models.cuh"
 #include "state.h"
@@ -259,8 +259,7 @@ int BuildSharedTablesLocked(int device, SharedTables& g_tables) {
   CK(cudaMemcpyToSymbol(c_ivmap, ivmap, sizeof ivmap));
   CK(cudaMemcpyToSymbol(c_mixer_sel, msel, sizeof msel));
   CK(cudaFuncSetAttribute(small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallState)));
-  CK(cudaFuncSetAttribute(mix_kernel_v3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MixShared3)));
-  CK(cudaFuncSetAttribute(mix_predict_final_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MixShared)));
+  CK(cudaFuncSetAttribute(mix_kernel_v3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MixBulkShared)));
   CK(cudaFuncSetAttribute(lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LstmShared)));
   CK(cudaFuncSetAttribute(ppmd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(PPMD_WARPS * sizeof(PpmdWarpShared))));
   CK(cudaFuncSetAttribute(lstm_byte_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LstmShared)));
@@ -735,7 +734,7 @@ int LaunchChunk(cmixb200_predictor* lead, ChunkArgs* d_args, int n_streams, bool
     CK(cudaStreamWaitEvent(lead->s_mix, lead->ev[1], 0));
     CK(cudaStreamWaitEvent(lead->s_mix, lead->ev[2], 0));
     { cudaEvent_t t = tick(lead->s_mix);
-    mix_kernel_v3<<<2 * n_streams, MIX_THREADS, sizeof(MixShared3), lead->s_mix>>>(d_args, T);
+    mix_kernel_v3<<<2 * n_streams, MIX_THREADS, sizeof(MixBulkShared), lead->s_mix>>>(d_args, T);
     tock(0, t, lead->s_mix); }
     lead->launches++;
     if (with_coder) { encode_kernel<<<n_streams, 32, 0, lead->s_mix>>>(d_args); lead->launches++; }
@@ -972,7 +971,7 @@ static int LaunchPredict(cmixb200_predictor* P) {
   CK(cudaStreamWaitEvent(P->s_mix, P->ev_lock_small, 0));
   if (P->d_p8) CK(cudaStreamWaitEvent(P->s_mix, P->ev_lock_p8, 0));
   mix_predict_rows_kernel<<<N_L0, 256, 0, P->s_mix>>>(P->d_st, T, (P->ext_bit_valid || P->d_fx || P->d_p8) ? P->d_ext_bit.p : nullptr);
-  mix_predict_final_kernel<<<1, MIX_THREADS, sizeof(MixShared), P->s_mix>>>(P->d_st, T);
+  mix_predict_final_kernel<<<1, MIX_THREADS, 0, P->s_mix>>>(P->d_st, T);
   P->launches += 3;
   return CMIXB200_OK;
 }

@@ -57,15 +57,19 @@ struct MixerState {
 };
 
 // ---- final SSE stage (reference mixer/sse.cpp) ----
+// What SSE's estimate leaves for its update (M_T::su6/su7/mix*, sse.cpp:243-305): interpolation and mixing terms.
+struct SseCarry {
+  int sw6, q6, P6, sw7, q7, P7;
+  int s0, s1, sm, s4, mix1_p, mix2_p;
+};
 struct SseState {
   u16* s6; u16* s7;     // [vol][7] interpolation buckets (padded to 8 u16 per bucket set)
   int* x1; int* x2;     // 1-weight integer mixers
   u16* st; u16* sq;     // stretch / squash tables (32768 each, host-built with libm)
   u32 j, pc, ffl;
-  // carried from Predict to Perceive (M_T::su6/su7/mix*)
-  u32 sm6x, sm7x, mix1, mix2;
-  int sw6, sw7, P6, P7, q6, q7;
-  int mix1_s0, mix1_s1, mix1_p, mix2_s0, mix2_s1, mix2_p;
+  // carried from Predict to Perceive: the bucket sets and weights the estimate used, and its terms
+  u32 i6, i7, ix1, ix2;
+  SseCarry c;
 };
 
 // ---- small models + shared contexts (reference context-manager.cpp, contexts/, models/) ----

@@ -20,5 +20,5 @@ prof8 = prof[8]
 for i, nm in enumerate(names):
     print('%-18s %8.0f cycles/byte' % (nm, prof[32 + i] / bits * 8))
 print('LSTM total         %8.0f cycles/byte' % (prof[32:43].sum() / bits * 8))
-v2 = {8:'C0 wait-ready',9:'C0 chain',10:'C0 recv',11:'C0 extras',12:'C0 coeff',13:'C0 publish',14:'C1 wait-ready',15:'C1 chain',16:'C1 recv',17:'C1 extras',18:'C1 coeff',19:'C1 publish',20:'M stage',21:'M aux+plan',22:'M jobs+rate',23:'M late path',24:'M wait-coeff',25:'M update',26:'T prefetch',27:'T wait-ring',28:'T layer1',29:'T layer2+SSE',30:'T update'}
-for k in sorted(v2): print('%-18s %8.0f cycles/bit' % (v2[k], prof[k] / bits))
+phases = {8:'C0 wait-ready',9:'C0 chain',10:'C0 recv',11:'C0 extras',12:'C0 coeff',13:'C0 publish',14:'C1 wait-ready',15:'C1 chain',16:'C1 recv',17:'C1 extras',18:'C1 coeff',19:'C1 publish',20:'M stage',21:'M aux+plan',22:'M jobs+rate',23:'M late path',24:'M wait-coeff',25:'M update',26:'T prefetch',27:'T wait-ring',28:'T layer1',29:'T layer2+SSE',30:'T update'}
+for k in sorted(phases): print('%-18s %8.0f cycles/bit' % (phases[k], prof[k] / bits))
