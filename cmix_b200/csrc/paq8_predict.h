@@ -91,7 +91,8 @@ struct TextM {   // TextModel (:3070-3519)
 };
 struct DetectM {   // the header detectors in front of the image / audio / JPEG models (:5386-5509, :5810-5870, :6031-6060)
   int bmp_header, bmp_offset, bmp_hdrless, bmp_bitmask, tga_header, tga_id, tga_map, tga_bpp, tga_type, tga_w, tga_h, eoi, w;
-  u32 wav_header, wav_eoi;
+  u32 wav_header, wav_channels, wav_bits, wav_chunk;   // audioModel's WAVAudio (:5806-5808)
+  u32 wav_length, wav_eoi, wav_info;                   // and its statics `length`, `eoi`, `info` (:5811)
 };
 
 struct State {

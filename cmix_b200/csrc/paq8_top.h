@@ -716,6 +716,46 @@ P8_HD inline void linear_bit(State& S, Out& o) {
 P8_HD inline u32 le4(const State& S, int i) { return (u32)buf(S, i) + 256u * (u32)buf(S, i - 1) + 65536u * (u32)buf(S, i - 2) + 16777216u * (u32)buf(S, i - 3); }
 P8_HD inline int le2(const State& S, int i) { return buf(S, i) + 256 * buf(S, i - 1); }
 P8_HD inline u32 be4(const State& S, int i) { return (u32)buf(S, i - 3) + 256u * (u32)buf(S, i - 2) + 65536u * (u32)buf(S, i - 1) + 16777216u * (u32)buf(S, i); }
+// audioModel's parser (:5811-5866), run at the start of every byte: the WAVAudio header state, `length`, `eoi` and `info`.
+// info != 0 is audio mode: on those bytes the reference runs audio8bModel / wavModel and recordModel(AUDIO) instead of the
+// ordinary models. They are not built, so audio mode raises ERR_UNSUPPORTED_BLOCK; it starts on the first byte of a PCM data
+// chunk whose length is a whole number of sample blocks. Any other RIFF stream (AVI, WebP, compressed or 24-bit WAV,
+// truncated headers, "RIFF" in text) codes with the ordinary models.
+P8_HD inline void wav_byte(State& S) {
+  DetectM& D = S.detect;
+  // the reference clears WAVAudio on bit 7 of the byte before eoi (:5865-5866); nothing reads it in between
+  if (S.pos > 0 && S.pos == (int)D.wav_eoi) D.wav_header = D.wav_channels = D.wav_bits = D.wav_chunk = 0;
+  if (S.pos >= (int)(D.wav_eoi + 4) && !D.wav_header && be4(S, 4) == 0x52494646u) {   // "RIFF"
+    D.wav_header = (u32)S.pos; D.wav_chunk = 0; D.wav_length = 0;
+  } else if (D.wav_header) {
+    const int p = S.pos - (int)D.wav_header;
+    const u32 len = D.wav_length;
+    if (p == 4) D.wav_header *= (le4(S, 4) <= 0x3FFFFFFFu);
+    else if (p == 8) D.wav_header *= (be4(S, 4) == 0x57415645u);   // "WAVE"
+    else if (p == (int)(16 + len) && (be4(S, 8) != 0x666d7420u || ((D.wav_chunk = le4(S, 4) - 16) & 0xFFFFFFFDu) != 0)) {   // "fmt " of 16 or 18 bytes
+      D.wav_length = ((le4(S, 4) + 1) & ~1u) + 8;
+      D.wav_header *= !(be4(S, 8) == 0x666d7420u && (le4(S, 4) & 0xFFFFFFFDu) != 16);
+    } else if (p == (int)(20 + len)) {   // PCM, 1 or 2 channels
+      D.wav_channels = (u32)buf(S, 2);
+      D.wav_header *= ((D.wav_channels == 1 || D.wav_channels == 2) && (be4(S, 4) & 0xFFFFFCFFu) == 0x01000000u);
+    } else if (p == (int)(32 + len)) {   // 8 or 16 bits per sample
+      D.wav_bits = (u32)buf(S, 2);
+      D.wav_header *= ((D.wav_bits == 8 || D.wav_bits == 16) && ((buf(S, 2) * 256 + buf(S, 1)) & 0xE7FF) == 0);
+    } else if (p == (int)(40 + len + D.wav_chunk) && be4(S, 8) != 0x64617461u) {   // a chunk other than "data": skip it
+      D.wav_chunk += ((le4(S, 4) + 1) & ~1u) + 8;
+      D.wav_header *= (D.wav_chunk <= 0xFFFFFu);
+    } else if (p == (int)(40 + len + D.wav_chunk)) {
+      // block is 0 only on headers where the reference divides by zero (channels or bits never read); those stay ordinary data
+      const u32 data = (le4(S, 4) + 1) & ~1u, block = D.wav_channels * (D.wav_bits / 8);
+      if (data && block && data % block == 0) {
+        D.wav_info = (D.wav_channels + D.wav_bits / 4 - 3) + 1;
+        D.wav_eoi = (u32)S.pos + data;
+      }
+    }
+  }
+  if (S.pos > (int)D.wav_eoi) D.wav_info = 0;
+  if (D.wav_info) S.error |= ERR_UNSUPPORTED_BLOCK;
+}
 P8_COLD P8_HD inline void detect_byte(State& S) {
   // JPEG: SOI followed by a plausible marker (:6046-6049)
   if (S.filetype != FT_EXE && buf(S, 4) == 0xFF && buf(S, 3) == 0xD8 && buf(S, 2) == 0xFF &&
@@ -735,8 +775,7 @@ P8_COLD P8_HD inline void detect_byte(State& S) {
           ((be4(S, 8) & 0xFFFEFF) == 0x000200 && !be4(S, 4))) S.error |= ERR_UNSUPPORTED_BLOCK;
     }
   }
-  // WAV: "RIFF" (:5816)
-  if (S.pos >= 4 && be4(S, 4) == 0x52494646) S.error |= ERR_UNSUPPORTED_BLOCK;
+  wav_byte(S);
 }
 
 // ---------------------------------------------------------------- contextModel2 (:8101-8206) and Predictor::update (:8248-8362)

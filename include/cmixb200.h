@@ -24,7 +24,7 @@ extern "C" {
 
 enum { CMIXB200_OK = 0, CMIXB200_ERR_CUDA = 1, CMIXB200_ERR_ARG = 2,
        CMIXB200_ERR_CAPACITY = 3 /* a model arena is full (PPMD: raise CMIXB200_PPMD_MB); the stream is unusable */,
-       CMIXB200_ERR_UNSUPPORTED = 4 /* the resident PAQ8 met an image / audio / JPEG block it does not model; the stream is unusable */ };
+       CMIXB200_ERR_UNSUPPORTED = 4 /* the resident PAQ8 met an image / PCM WAV audio / JPEG block it does not model; the stream is unusable */ };
 
 enum {
   CMIXB200_N_EXT = 2022,  /* replayed FXCM (431) + PAQ8 (1591) outputs per bit, as 12-bit codes k

@@ -81,6 +81,7 @@ int main(int argc, char** argv) {
   std::vector<uint32_t> crcs;
   uint32_t crc = 0;
   size_t bad_bits = 0;
+  bool unsupported = false;
   for (size_t pos = 0; pos < n_bytes; ++pos) {
     for (int j = 7; j >= 0; --j) {
       const size_t t = pos * 8 + (7 - j);
@@ -105,10 +106,17 @@ int main(int argc, char** argv) {
 #ifdef CENSUS
       census::end_bit();
 #endif
-      if (S->error) { fprintf(stderr, "model raised error %u at bit %zu (unsupported block type)\n", S->error, t); printf("UNSUPPORTED after %zu bits\n", t); return 3; }
+      if (S->error) {
+        fprintf(stderr, "model raised error %u at bit %zu (unsupported block type)\n", S->error, t);
+        printf("UNSUPPORTED after %zu bits\n", t);
+        unsupported = true;   // the CRCs of the blocks completed before the error are still written
+        n_bytes = pos;
+        break;
+      }
     }
   }
   if (crc_out) { FILE* f = fopen(crc_out, "wb"); fwrite(crcs.data(), 4, crcs.size(), f); fclose(f); }
+  if (unsupported) return 3;
 #ifdef CENSUS
   census::print(stdout, {{"sparse", &S->sparse.cm}, {"sparse1", &S->sparse1.cm}, {"distance", &S->distance.cm}, {"record.cm", &S->record.cm},
                          {"record.cn", &S->record.cn}, {"record.co", &S->record.co}, {"record.cp", &S->record.cp}, {"record1.cm", &S->record1.cm},
