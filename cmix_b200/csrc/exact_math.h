@@ -14,8 +14,9 @@
 //          routines that glibc adopted in 2.27 (three multiply-adds contracted
 //          to FMA in the x86-64 FMA build),
 //   tanhf/expm1f : the single-precision fdlibm algorithms.
-// tests/test_exact_math.py pins them against the host libm over dense sweeps
-// (and tools/exact_math_sweep.cpp over all 2^32 inputs).
+// tests/test_exact_math_device.py checks the device build against the host build over all 2^32 inputs
+// (tests/exact_math_sweep.cu / .cpp), and the host build against glibc on the special classes (all 2^32
+// inputs with CMIXB200_SLOW=1).
 //
 // Every operation is written with explicit rounding intrinsics so nvcc can
 // never contract a multiply-add that the oracle does not contract.

@@ -92,7 +92,7 @@ def test_port_is_deterministic_and_learns(port):
 
 def test_exact_math_matches_libm(port, tmp_path):
     """cmix_b200/csrc/exact_math.h (host build) == glibc expf/tanhf on a dense sample.
-    (tools/exact_math_sweep.cpp checks all 2^32 inputs; 0 mismatches recorded in DESIGN.md.)"""
+    (tests/test_exact_math_device.py checks all 2^32 inputs; 0 mismatches recorded in DESIGN.md.)"""
     src = tmp_path / "xm.cpp"
     src.write_text('#include "%s/cmix_b200/csrc/exact_math.h"\n'
                    'extern "C" float t_expf(float x){return xm_expf(x);} extern "C" float t_tanhf(float x){return xm_tanhf(x);}\n'
