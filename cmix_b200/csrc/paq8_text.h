@@ -592,12 +592,32 @@ struct StemDE {
     }
   }
   P8_HD static bool valid_ending(int c, bool with_r = false) { return in_set(c, "bdfghklmnt") || (with_r && c == 'r'); }
+  P8_HD static void move(u8* L, int d, int s, int n) { u8 t[8]; for (int k = 0; k < n; ++k) t[k] = L[s + k]; for (int k = 0; k < n; ++k) L[d + k] = t[k]; }
+  // GermanStemmer::ConvertUTF8 closes the gap with memcpy(&L[d], &L[d + 1], n) (paq8.cpp:2851): source and destination
+  // overlap, so the result is whatever the compiled copy does. g++ -O2, the build the reference's outputs come from, expands
+  // it inline: whole 8/4/2/1-byte loads and stores, the tail chunk after the head, then 8-byte words from the first 8-aligned
+  // destination (the word's letters are 8-aligned). A word of 5-8 bytes after the umlaut thereby loses a letter and repeats
+  // its last one (m ü l l e r -> m ü l e r r). Restated step for step.
+  P8_HD static void close_gap(u8* L, int d, int n) {
+    if (n >= 8) {
+      move(L, d, d + 1, 8);
+      move(L, d + n - 8, d + 1 + n - 8, 8);
+      const int a = 8 - (d & 7);
+      for (int k = 0; k < ((n - a) >> 3); ++k) move(L, d + a + 8 * k, d + 1 + a + 8 * k, 8);
+    } else if (n & 4) {
+      move(L, d, d + 1, 4);
+      move(L, d + n - 4, d + 1 + n - 4, 4);
+    } else if (n) {
+      move(L, d, d + 1, 1);
+      if (n & 2) move(L, d + n - 2, d + 1 + n - 2, 2);
+    }
+  }
   P8_HD static bool stem(Word& w) {
     for (int i = w.s; i < w.e; ++i) {   // ConvertUTF8
       const u8 c = (u8)(w.L[i + 1] + ((w.L[i + 1] < 0x9F) ? 0x60 : 0x40));
       if (w.L[i] == 0xC3 && (vowel(c) || c == 0xDF)) {
         w.L[i] = c;
-        if (i + 1 < w.e) for (int k = 0; k < w.e - i - 1; ++k) w.L[i + 1 + k] = w.L[i + 2 + k];
+        if (i + 1 < w.e) close_gap(w.L, i + 1, w.e - i - 1);
         w.e--;
       }
     }

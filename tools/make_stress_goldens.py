@@ -22,19 +22,20 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
-from gen_stress import STREAMS, coded_stream, generate  # noqa: E402
+import gen_stress  # noqa: E402
 from oracle_io import Dump  # noqa: E402
 
 ORACLE = os.path.join(ROOT, "oracle", "_ref", "oracle_dump")
 
 
-def make(name, tmp):
-    n, seed = STREAMS[name]
+def make(name, tmp, gen=gen_stress, kind="stress"):
+    """tests/golden/<kind>_<name>.npz from stream `name` of generator module `gen` (gen_stress or gen_reach)."""
+    n, seed = gen.STREAMS[name]
     src, prefix = os.path.join(tmp, name + ".bin"), os.path.join(tmp, name)
-    generate(name, n, seed).tofile(src)
+    gen.generate(name, n, seed).tofile(src)
     subprocess.run([ORACLE, "dump", "n", src, prefix, "1", str(n)], check=True)
     d = Dump(prefix)
-    assert d.n_bytes == n and n % 512 == 0 and np.array_equal(d.stream, coded_stream(name))
+    assert d.n_bytes == n and n % 512 == 0 and np.array_equal(d.stream, gen.coded_stream(name))
     nb = n * 8
     ext = d.ext
     crc_fx = np.array([zlib.crc32(np.ascontiguousarray(ext[b:b + 4096, :431]).tobytes()) for b in range(0, nb, 4096)], dtype=np.uint32)
@@ -42,7 +43,7 @@ def make(name, tmp):
     ppmd_crc = np.array([zlib.crc32(d.ppmd[t].tobytes()) for t in range(n)], dtype=np.uint32)
     lstmfx = np.fromfile(prefix + ".lstmfx.u32", dtype=np.uint32)
     assert lstmfx.size == nb
-    out = os.path.join(ROOT, "tests", "golden", "stress_%s.npz" % name)
+    out = os.path.join(ROOT, "tests", "golden", "%s_%s.npz" % (kind, name))
     np.savez_compressed(out, stream=d.stream, vocab=d.vocab, p=d.p, crc_fx=crc_fx, crc_p8=crc_p8, first_codes=np.ascontiguousarray(ext[:64]),
                         lstmfx=lstmfx, ppmd_crc=ppmd_crc, mode=np.array([d.meta["mode"]]), dictionary=np.array([0]))
     bits = np.unpackbits(d.stream)
@@ -50,10 +51,10 @@ def make(name, tmp):
     return "%-8s %5d bytes  %.3f bits/byte -> %d KiB" % (name, n, bpb, os.path.getsize(out) // 1024)
 
 
-def main():
-    names = sys.argv[1:] or list(STREAMS)
+def main(gen=gen_stress, kind="stress"):
+    names = sys.argv[1:] or list(gen.STREAMS)
     with tempfile.TemporaryDirectory() as tmp, ThreadPoolExecutor(4) as ex:
-        for line in ex.map(lambda k: make(k, tmp), names):
+        for line in ex.map(lambda k: make(k, tmp, gen, kind), names):
             print(line)
 
 

@@ -40,3 +40,29 @@ int ppmd_host_run(const unsigned char* stream, size_t n, const unsigned char* vo
 }
 
 }  // extern "C"
+
+#ifdef PPMD_HOST_MAIN
+// ppmd_host <stream file> <vocabulary file (256 bytes)>: the same run as a program, for the line-coverage build of
+// tools/coverage_report.py. Returns ppmd_host_run's code.
+#include <cstdio>
+#include <vector>
+
+static std::vector<unsigned char> slurp(const char* path) {
+  std::vector<unsigned char> v;
+  FILE* f = fopen(path, "rb");
+  if (!f) return v;
+  fseek(f, 0, SEEK_END); long n = ftell(f); fseek(f, 0, SEEK_SET);
+  v.resize(n);
+  if (n && fread(v.data(), 1, n, f) != (size_t)n) v.clear();
+  fclose(f);
+  return v;
+}
+
+int main(int argc, char** argv) {
+  if (argc < 3) { fprintf(stderr, "usage: ppmd_host <stream> <vocabulary>\n"); return 2; }
+  std::vector<unsigned char> stream = slurp(argv[1]), vocab = slurp(argv[2]);
+  if (stream.empty() || vocab.size() != 256) { fprintf(stderr, "ppmd_host: bad input\n"); return 2; }
+  std::vector<float> out(stream.size() * 256);
+  return ppmd_host_run(stream.data(), stream.size(), vocab.data(), out.data(), 64);
+}
+#endif
