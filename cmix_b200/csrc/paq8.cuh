@@ -12,11 +12,13 @@
 //    draws 24 at a time (the generator is a lagged XOR: x[i] = x[i-24] ^ x[i-55]); pass 2 applies them. A bit with a
 //    clashing map falls back to one lane walking the maps in order.
 //  * the match models, the DMC forest, the run maps and the direct maps run one unit per lane on warps 9-11 beside the
-//    context maps; on a bit inside a byte all of this is three phases (probe / number / apply). Byte boundaries add the
-//    context hashing of the word / nest / indirect / XML / text / x86 / record models (model per lane, two rounds because
-//    the sparse and record models consume what the order-N map and the match model produce in the same bit) and the three
-//    OLS predictors (one warp each: rank-1 covariance update with coalesced columns, Cholesky with a row per lane in
-//    registers, substitutions in the reference's summation order).
+//    context maps; on a bit inside a byte all of this is three phases (probe / number / apply). The bit that starts a byte
+//    first computes the new contexts, as chains of warps that do not wait for each other: the D-chain (order-N and x86
+//    contexts, their history maps, the match model, then the sparse and record models, which consume what the order-N map
+//    and the match model produce in the same bit), the word model, the text model with its stemmers, the three OLS
+//    predictors (one warp each: rank-1 covariance update with coalesced columns, Cholesky with a row per lane in
+//    registers, substitutions in the reference's summation order) and the nest / indirect / XML / distance / record1
+//    models. They meet once, before the common probe / number / apply of the sixteen 7-slot maps.
 //  * the mixer and the SSE stage run one or more bits behind the models on a second CTA of a 2-CTA cluster (nothing the
 //    models compute reads them back: the mixer's output feeds only the SSE stage, `st_misses` and selector set 26). The
 //    model CTA (rank 0) hands each bit over through a ring of P8_RING slots in the mixer CTA's shared memory (inputs,
@@ -40,8 +42,10 @@ namespace cmixb200 {
 enum { P8_SEEN = 4096, P8_RING = 4 };
 
 // -DP8_PROF: lane 0 of each CTA accumulates the cycles between phase boundaries (byte-boundary bits and the others apart):
-// slots 0-11 the model CTA (10: waiting for a free ring slot), 16-19 the mixer CTA (16: waiting for a full one), 24+ per-warp
-// times of the model phases
+// slots 0-11 the model CTA (2: from the end of the bookkeeping to the join of a byte boundary's chains, 10: waiting for a free
+// ring slot), 16-19 the mixer CTA (16: waiting for a full one). 24+: inside a byte the per-warp times of the probe (24 + warp)
+// and apply (48 + warp) phases; on a byte boundary the time from the end of the bookkeeping at which a chain got to a point
+// (24-30: warps 0-6 done, 31-36: the D-chain's steps, 38: the text chain done; labels in tools/prof_build.py)
 #ifdef P8_PROF
 __device__ unsigned long long g_p8_prof[2][96];
 #define P8_T(k) do { if (tid == 0) { const long long now_ = clock64(); atomicAdd(&g_p8_prof[sh.prof_row][k], (unsigned long long)(now_ - sh.prof_t)); sh.prof_t = now_; } } while (0)
@@ -56,6 +60,17 @@ __device__ unsigned long long g_p8_prof[2][96];
 #endif
 enum { P8_THREADS = 512, P8_WARPS = 16, P8_MAP_THREADS = 384, P8_MAP_WARPS = 12, P8_N_CM = 16, P8_N_CM2 = 3, P8_CM_LANES = 210, P8_CM2_LANES = 63, P8_N_UNITS = 53,
        P8_CM2_TID0 = 224, P8_TID_PIC = 287, P8_TID_MATCH = 288, P8_TID_W10 = 320, P8_TID_W11 = 352 };
+// Who computes the new contexts on the bit that starts a byte. A long single-lane job has a warp to itself while it runs
+// (lanes of one warp that diverge into different jobs run one after another):
+//   warps 0-2    the OLS predictors, lane 0 then the direct map behind its prediction
+//   warp 3       XML (lane 0)                     warp 4   distance, record1 (lane 0)
+//   warp 5       the word model: state and stemmer on lane 0, the 57 contexts on all lanes
+//   warp 6       nest, indirect, the two fixed linear predictions and their maps (lane 0)
+//   warps 7-11   the D-chain: order-N contexts (lane 0 of 7) and x86 contexts (lane 0 of 9); probe and apply of those two
+//                history maps with the single-lane units; then sparse (lane 0 of 9), sparse1 (lane 0 of 10), record (lane 0 of 11)
+//   warp 12      ModelStats and selector sets, as on every bit
+//   warps 13-15  the text chain: state on lane 0 of 13, a stemmer on lane 0 of each, the 33 contexts on warp 13
+// Then all of warps 0-11 as inside a byte, with the text history map's lanes (warps 7-8) beside the 7-slot maps.
 
 // One bit handed from the model CTA to the mixer CTA: what the models produced and the context the SSE stage reads.
 struct P8Slot {
@@ -83,7 +98,7 @@ struct P8Shared {
   u32 ids2[P8_CM2_LANES][5];
   int clash[P8_N_CM], clash2[P8_N_CM2];
   int order, res2[P8_N_CM2];
-  u32 snap_spaces, snap_words, snap_frstchar, snap_spafdo;
+  p8::WordStats snap;          // the word statistics as the byte found them (sparseModel1 reads them beside the word model's update)
   int dmc_st[10];
   u32 flag_mask[8];            // ballot of "this context draws" per warp of map lanes
   int flag_base[P8_N_CM];      // index of a map's first draw in draws[]
@@ -91,8 +106,10 @@ struct P8Shared {
   u32 rnd_prev[64]; int rnd_prev_i;   // the generator as the bit found it: flagged contexts compute their own draw from it
   int any_clash, text_pending;
   union {
-    unsigned long long seen[P8_SEEN];   // open-addressing set of (map, bucket) pairs touched this bit
-    struct { double ch[3][32 * 33]; double pb[3][32]; } ols;   // Cholesky factor rows (padded) and a product buffer; byte boundaries only
+    struct {                                                    // the model CTA
+      unsigned long long seen[P8_SEEN];   // open-addressing set of (map, bucket) pairs touched this bit
+      struct { double ch[3][32 * 33]; double pb[3][32]; } ols;   // Cholesky factor rows (padded) and a product buffer; byte boundaries only
+    } md;
     struct {                                                    // the mixer CTA
       alignas(16) short wc[p8::N_SETS][p8::N_IN];   // the weight sets of the pending prediction (slot i holds set wc_set[i])
       P8Slot ring[P8_RING];
@@ -154,7 +171,7 @@ __device__ __noinline__ void p8_ols_byte_warp(P8Shared& sh, int k, int lane) {
   const double lambda = 0.995, nu = 0.001, one_minus = 1.0 - 0.995;
   double* blk = M.ols + (size_t)k * OLS_STRIDE;
   double* x = blk; double* w = blk + 32; double* b = blk + 64; double* cov = blk + 96;
-  double* chs = sh.u.ols.ch[k]; double* pb = sh.u.ols.pb[k];
+  double* chs = sh.u.md.ols.ch[k]; double* pb = sh.u.md.ols.pb[k];
   double* row = chs + lane * 33;
   const unsigned full = 0xffffffffu;
   const double val = (double)(u8)buf(S, 1);
@@ -278,13 +295,13 @@ __device__ __forceinline__ int p8_flags_in(const u32* mask, int lo, int hi) {
 
 // ---- the pieces of a bit ----------------------------------------------------------------------------------------------
 // probe of the history maps (lanes P8_CM2_TID0 ..): buckets each context touches this bit
-__device__ __noinline__ void p8_probe_cm2(P8Shared& sh, int tid, int bpos) {
+__device__ __noinline__ void p8_probe_cm2(P8Shared& sh, int tid, int bpos, int maps) {   // maps: bit k set = history map k
   int k, i;
-  if (!p8_cm2_lane(tid - P8_CM2_TID0, k, i)) return;
+  if (!p8_cm2_lane(tid - P8_CM2_TID0, k, i) || !(maps >> k & 1)) return;
   p8::Cm2& m = p8_cm2(sh.S, k);
   u32* ids = sh.ids2[tid - P8_CM2_TID0];
   const int n = i < m.index ? p8::cm2_touched(m, i, bpos, ids) : 0;
-  if (n && p8_claim(sh.u.seen, P8_N_CM + k, ids, n)) sh.clash2[k] = 1;
+  if (n && p8_claim(sh.u.md.seen, P8_N_CM + k, ids, n)) sh.clash2[k] = 1;
 }
 // pass 1 of the 7-slot maps (warps 0-6, whole warps): aged state, draw flag, touched buckets
 __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, int bpos) {
@@ -297,7 +314,7 @@ __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, i
     if (i < m.cn) {
       ns = cm_next_state(*sh.S.T, m, i, y);
       const int n = cm_touched(m, i, c0, bpos, sh.ids[tid]);
-      if (p8_claim(sh.u.seen, k, sh.ids[tid], n)) { sh.clash[k] = 1; sh.any_clash = 1; }
+      if (p8_claim(sh.u.md.seen, k, sh.ids[tid], n)) { sh.clash[k] = 1; sh.any_clash = 1; }
     }
     sh.ns[tid] = (short)ns;
     flag = ns >= 204;
@@ -312,13 +329,15 @@ __device__ __noinline__ void p8_probe_single(P8Shared& sh, int tid, int y, int c
   const p8::Tables& T = *S.T;
   if (tid == P8_TID_PIC) pic_core(S);
   else if (tid == P8_TID_MATCH) { Out o = p8_out(sh, sh.unit_off[7]); match_core(S, o); }
-  else if (tid == P8_TID_MATCH + 1) { if (bpos != 0) record_pre(S); }   // on a byte boundary it follows record_byte (round 2)
+  else if (tid == P8_TID_MATCH + 1) { if (bpos != 0) record_pre(S); }   // on a byte boundary it follows record_byte
   else if (tid >= P8_TID_W10 && tid < P8_TID_W10 + 10) sh.dmc_st[tid - P8_TID_W10] = dmc_st(T, S.dmc[tid - P8_TID_W10], y);
   else if (tid >= P8_TID_MATCH + 2 && tid < P8_TID_MATCH + 5) {
     const int r = tid - (P8_TID_MATCH + 2);
     Out o = p8_out(sh, sh.unit_off[4 + r]);
     rcm_mix(r == 0 ? S.rcm7 : r == 1 ? S.rcm9 : S.rcm10, o, c0, bpos);
-  } else if (tid >= P8_TID_W11 + 4 && tid < P8_TID_W11 + 9) { const int r = tid - (P8_TID_W11 + 4); Out o = p8_out(sh, sh.unit_off[48 + r]); linear_small(S, o, r); }
+  } else if (tid >= P8_TID_W11 + 4 && tid < P8_TID_W11 + 9) {   // on a byte boundary each follows its predictor
+    if (bpos != 0) { const int r = tid - (P8_TID_W11 + 4); Out o = p8_out(sh, sh.unit_off[48 + r]); linear_small(S, o, r); }
+  }
   else if (tid == P8_TID_W11) { Out o = p8_out(sh, sh.unit_off[8]); smatch_head(S, o); }
   else if (tid == P8_TID_W11 + 1 || tid == P8_TID_W11 + 2) {
     const int r = tid - (P8_TID_W11 + 1);
@@ -370,9 +389,9 @@ __device__ __noinline__ void p8_number(P8Shared& sh, int tid, int y, int c0, int
   }
 }
 // pass 2
-__device__ __noinline__ void p8_apply_cm2(P8Shared& sh, int tid, int y, int bpos) {
+__device__ __noinline__ void p8_apply_cm2(P8Shared& sh, int tid, int y, int bpos, int maps) {
   int k, i;
-  if (!p8_cm2_lane(tid - P8_CM2_TID0, k, i)) return;
+  if (!p8_cm2_lane(tid - P8_CM2_TID0, k, i) || !(maps >> k & 1)) return;
   p8::Cm2& m = p8_cm2(sh.S, k);
   const int off = sh.unit_off[c_p8_cm2_unit[k]];
   if (!sh.clash2[k]) {
@@ -508,6 +527,20 @@ static_assert(p8::N_IN % 8 == 0 && p8::N_IN / 8 <= 7 * 32, "a weight row is at m
 __device__ __forceinline__ void p8_signal_selects() { asm volatile("bar.arrive 2, 416;" ::: "memory"); }
 __device__ __forceinline__ void p8_await_selects() { asm volatile("bar.sync 2, 416;" ::: "memory"); }
 __device__ __forceinline__ void p8_sync_maps() { asm volatile("bar.sync 1, 384;" ::: "memory"); static_assert(P8_MAP_THREADS == 384, "named barrier width"); }
+// The bit that starts a byte runs its context computation as independent chains of warps (p8_model_bit) ordered by three
+// more named barriers. Every arrive / sync below is executed by whole warps, unconditionally on that bit:
+//  3 (join, 480): "the new contexts of every map are set". Warps 0-11 sync on it before the probe of the 7-slot maps
+//                 (384), the text chain's warps 13-15 arrive (96) and go on to the end of the bit.
+//  4 (160):       the D-chain's warps 7-11 between its steps.
+//  5 (96):        the text chain's warps 13-15 between its steps.
+__device__ __forceinline__ void p8_join_sync() { asm volatile("bar.sync 3, 480;" ::: "memory"); }
+__device__ __forceinline__ void p8_join_arrive() { __threadfence_block(); asm volatile("bar.arrive 3, 480;" ::: "memory"); }
+__device__ __forceinline__ void p8_sync_dchain() { asm volatile("bar.sync 4, 160;" ::: "memory"); }
+__device__ __forceinline__ void p8_sync_text() { asm volatile("bar.sync 5, 96;" ::: "memory"); }
+enum { P8_WARP_D = P8_CM2_TID0 / 32, P8_WARP_TEXT = P8_MAP_WARPS + 1 };   // first warp of the D-chain / of the text chain
+static_assert(P8_CM2_TID0 % 32 == 0 && P8_CM_LANES <= P8_CM2_TID0 && (P8_MAP_WARPS - P8_WARP_D) * 32 == 160, "barrier 4: warps 7-11");
+static_assert((P8_WARPS - P8_WARP_TEXT) * 32 == 96 && P8_MAP_THREADS + 96 == 480, "barriers 3 and 5: warps 13-15 beside the 12 map warps");
+static_assert(P8_TID_MATCH == (P8_WARP_D + 2) * 32 && P8_TID_W10 == (P8_WARP_D + 3) * 32 && P8_TID_W11 == (P8_WARP_D + 4) * 32, "a warp per long job of the D-chain");
 
 // The ring's mbarriers. An arrive on the other CTA's barrier releases at cluster scope what the arriving thread wrote or
 // read before it; a wait acquires it.
@@ -566,7 +599,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
   if (tid == 0) {
     bit_begin(S, y);
     if (S.bpos == 0) block_parse(S);
-    sh.snap_spaces = S.spaces; sh.snap_words = S.words; sh.snap_frstchar = S.frstchar; sh.snap_spafdo = S.spafdo;
+    sh.snap = word_stats(S);
   }
   if (tid >= 32 && tid < 32 + P8_N_CM) sh.clash[tid - 32] = 0;
   if (tid >= 64 && tid < 64 + P8_N_CM2) { sh.clash2[tid - 64] = 0; sh.res2[tid - 64] = 0; }
@@ -587,7 +620,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     sh.unit_off[lane] = ia - a;
     if (lane + 32 <= P8_N_UNITS) sh.unit_off[lane + 32] = ta + ib - b;
   }
-  for (int k = tid; k < P8_SEEN; k += P8_THREADS) sh.u.seen[k] = 0ull;
+  for (int k = tid; k < P8_SEEN; k += P8_THREADS) sh.u.md.seen[k] = 0ull;
   __syncthreads();
   P8_T(0);
   const int bpos = S.bpos, c0 = S.c0;
@@ -604,16 +637,58 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         if (S.m.ncxt != MAIN_SET_FIRST || S.m.base != MAIN_SET_BASE) S.error |= ERR_MIXER_ALIAS;
         S.m.ncxt = N_SETS;
       }
+    } else if (byte_start) {
+      // ---- byte boundary, the text chain (warps 13-15): state on one lane, the three stemmers of a completed word a warp
+      // each, then the 33 contexts side by side. Nothing else reads the text model before the join.
+      P8_M0;
+      if (tid == P8_WARP_TEXT * 32) sh.text_pending = text_update_a(S);
+      p8_sync_text();
+      if (sh.text_pending) {
+        const int split = S.text.stem_split;
+        const int i = warp == P8_WARP_TEXT ? LANG_EN : (warp == P8_WARP_TEXT + 1 ? LANG_FR : LANG_DE);
+        if (lane == 0 && i >= split) text_stem(S, i);
+        p8_sync_text();
+        if (tid == P8_WARP_TEXT * 32) {
+          text_stem_mid(S);
+          for (int j = split - 1; j > LANG_UNKNOWN; --j) text_stem(S, j);
+          text_update_b(S);
+        }
+      }
+      if (warp == P8_WARP_TEXT) {
+        __syncwarp();
+        const int n = text_contexts(S, CtxSel{lane, 32});
+        __syncwarp();
+        if (lane == 0) { S.text.map.index = n; P8_M(38); }
+      }
+      p8_join_arrive();
     }
   } else {
     if (tid == 0) { S.m.nx = S.m.base = S.m.ncxt = 0; }
     if (byte_start) {
-      // ---- byte boundary, round 1: context computation, one model per lane / warp
+      // ---- byte boundary: the new contexts, as chains of warps that meet at the join (lane map: DESIGN 4.5)
       {
         P8_M0;
-        if (warp < 3) p8_ols_byte_warp(sh, warp, lane);
-        else if (warp == 8) {       // the text model: state on one lane (the stemmers of a completed word follow below)
-          if (lane == 0) sh.text_pending = text_update_a(S);
+        if (warp >= P8_WARP_D) {
+          // the D-chain: order-N and x86 contexts -> their history maps and the single-lane units -> the sparse and record
+          // models, which consume the order-N map's result and the match length of this bit
+          if (tid == P8_CM2_TID0) ordern_byte(S);
+          else if (tid == P8_TID_MATCH) exe_byte(S);
+          p8_sync_dchain();
+          if (tid == P8_CM2_TID0) P8_M(31);
+          p8_probe_cm2(sh, tid, bpos, 5);
+          p8_probe_single(sh, tid, y, c0, bpos);
+          p8_sync_dchain();
+          if (tid == P8_CM2_TID0) P8_M(32);
+          p8_apply_cm2(sh, tid, y, bpos, 5);
+          p8_sync_dchain();
+          if (tid == P8_CM2_TID0) P8_M(33);
+          const int ismatch = ilog(T, S.match.length);
+          if (tid == P8_TID_MATCH) { sparse_byte(S, ismatch, sh.res2[0]); P8_M(34); }
+          else if (tid == P8_TID_W10) { sparse1_byte(S, ismatch, sh.res2[0], sh.snap); P8_M(35); }
+          else if (tid == P8_TID_W11) { record_byte(S); record_pre(S); P8_M(36); }
+        } else if (warp < 3) {      // a linear predictor per warp, then the map behind it
+          p8_ols_byte_warp(sh, warp, lane);
+          if (lane == 0) { Out o = p8_out(sh, sh.unit_off[48 + warp]); linear_small(S, o, warp); }
         } else if (warp == 5) {     // the word model: state on one lane, its 57 contexts side by side
           if (lane == 0) word_update(S);
           __syncwarp();
@@ -622,73 +697,31 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
           if (lane == 0) { S.word.cm.cn = n; word_finish(S); }
         } else if (lane == 0) {
           switch (warp) {
-            case 3: ordern_byte(S); break;
+            case 3: xml_byte(S); break;
             case 4: distance_byte(S); record1_byte(S); break;
-            case 6: nest_byte(S); indirect_byte(S); break;
-            case 7: xml_byte(S); break;
-            case 9: exe_byte(S); break;
-            case 10: {
+            case 6: {
+              nest_byte(S); indirect_byte(S);
               const u8 W = (u8)buf(S, 1), WW = (u8)buf(S, 2), WWW = (u8)buf(S, 3);
               S.linear.prd[3] = (u8)clip8(W * 2 - WW);
               S.linear.prd[4] = (u8)clip8(W * 3 - WW * 3 + WWW);
+              for (int r = 3; r < 5; ++r) { Out o = p8_out(sh, sh.unit_off[48 + r]); linear_small(S, o, r); }
             } break;
           }
         }
-        if (lane == 0) P8_M(24 + warp);
+        if (lane == 0 && warp < P8_WARP_D) P8_M(24 + warp);
       }
-      p8_sync_maps();
-      if (sh.text_pending) {      // a word ended: its three stemmers on three warps, then the rest of the text model's byte
-        const int split = S.text.stem_split;
-        if (lane == 0 && (warp == 8 || warp == 10 || warp == 11)) {
-          const int i = warp == 8 ? LANG_EN : (warp == 10 ? LANG_FR : LANG_DE);
-          if (i >= split) text_stem(S, i);
-        }
-        p8_sync_maps();
-        if (tid == 8 * 32) {
-          text_stem_mid(S);
-          for (int i = split - 1; i > LANG_UNKNOWN; --i) text_stem(S, i);
-          text_update_b(S);
-        }
-        p8_sync_maps();
-      }
-      if (warp == 8) {            // the text model's 33 contexts side by side
-        const int n = text_contexts(S, CtxSel{lane, 32});
-        __syncwarp();
-        if (lane == 0) S.text.map.index = n;
-      }
-      P8_T(2);
-      for (int k = tid; k < P8_SEEN; k += P8_MAP_THREADS) sh.u.seen[k] = 0ull;   // the OLS warps used this memory
-      p8_sync_maps();
-      // ---- the history maps and the single-lane units
-      p8_probe_cm2(sh, tid, bpos);
-      p8_probe_single(sh, tid, y, c0, bpos);
-      p8_sync_maps();
-      P8_T(3);
-      p8_apply_cm2(sh, tid, y, bpos);
-      p8_sync_maps();
-      P8_T(4);
-      // ---- round 2 of the byte boundary (needs the order-N result and the match model)
-      {
-        const int ismatch = ilog(T, S.match.length);
-        if (tid == 32) sparse_byte(S, ismatch, sh.res2[0]);
-        else if (tid == 64) {
-          // sparseModel1 runs BEFORE wordModel in the reference: it sees the previous byte's word statistics
-          const u32 a = S.spaces, b = S.words, c = S.frstchar, d = S.spafdo;
-          S.spaces = sh.snap_spaces; S.words = sh.snap_words; S.frstchar = sh.snap_frstchar; S.spafdo = sh.snap_spafdo;
-          sparse1_byte(S, ismatch, sh.res2[0]);
-          S.spaces = a; S.words = b; S.frstchar = c; S.spafdo = d;
-        } else if (tid == 96) { record_byte(S); record_pre(S); }
-      }
-      for (int k = tid; k < P8_SEEN; k += P8_MAP_THREADS) sh.u.seen[k] = 0ull;
-      p8_sync_maps();
+      p8_join_sync();
       p8_signal_selects();
-      P8_T(5);
-      if (warp < 7) p8_probe_cm(sh, tid, y, c0, bpos);
+      P8_T(2);
+      // ---- the sixteen 7-slot maps in one probe / number / apply (their random draws are shared), the text history map beside them
+      if (warp < P8_WARP_D) p8_probe_cm(sh, tid, y, c0, bpos);
+      else p8_probe_cm2(sh, tid, bpos, 2);
       p8_sync_maps();
       P8_T(6);
       if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(); }
       P8_T(7);
       p8_apply_cm(sh, tid, y, c0, bpos);
+      p8_apply_cm2(sh, tid, y, bpos, 2);
       p8_apply_small(sh, tid, y, bpos);
       p8_sync_maps();
       P8_T(8);
@@ -697,7 +730,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       {
         P8_M0;
         if (warp < 7) p8_probe_cm(sh, tid, y, c0, bpos);
-        else { p8_probe_cm2(sh, tid, bpos); p8_probe_single(sh, tid, y, c0, bpos); }
+        else { p8_probe_cm2(sh, tid, bpos, 7); p8_probe_single(sh, tid, y, c0, bpos); }
         __syncwarp();
         if (lane == 0) P8_M(24 + warp);
       }
@@ -709,7 +742,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       {
         P8_M0;
         if (warp < 7) p8_apply_cm(sh, tid, y, c0, bpos);
-        else { p8_apply_cm2(sh, tid, y, bpos); p8_apply_small(sh, tid, y, bpos); }
+        else { p8_apply_cm2(sh, tid, y, bpos, 7); p8_apply_small(sh, tid, y, bpos); }
         __syncwarp();
         if (lane == 0) P8_M(48 + warp);
       }

@@ -334,7 +334,11 @@ P8_COLD P8_HD inline void sparse_byte(State& S, int seenbefore, int howmany) {  
     cm_set(cm, hash(++i, (u64)((buf(S, j + 3) << 8) | buf(S, j + 1))));
   }
 }
-P8_COLD P8_HD inline void sparse1_byte(State& S, int seenbefore, int howmany) {   // :4539-4586
+// sparseModel1 runs BEFORE wordModel in the reference: it reads the word statistics of the previous byte. The caller passes them,
+// so that a device lane can run this beside the word model's state update.
+struct WordStats { u32 spaces, words, frstchar, spafdo; };
+P8_HD inline WordStats word_stats(const State& S) { WordStats w; w.spaces = S.spaces; w.words = S.words; w.frstchar = S.frstchar; w.spafdo = S.spafdo; return w; }
+P8_COLD P8_HD inline void sparse1_byte(State& S, int seenbefore, int howmany, const WordStats& W) {   // :4539-4586
   Sparse1M& M = S.sparse1;
   Cm& cm = M.cm;
   const u32 c4 = S.c4;
@@ -354,9 +358,9 @@ P8_COLD P8_HD inline void sparse1_byte(State& S, int seenbefore, int howmany) { 
     cm_set(cm, sx(seenbefore | buf(S, i) << 8));
     cm_set(cm, (u64)((buf(S, i + 3) << 8) | buf(S, i + 1)));
   }
-  cm_set(cm, S.spaces & 0x7fff);
-  cm_set(cm, S.spaces & 0xff);
-  cm_set(cm, S.words & 0x1ffff);
+  cm_set(cm, W.spaces & 0x7fff);
+  cm_set(cm, W.spaces & 0xff);
+  cm_set(cm, W.words & 0x1ffff);
   cm_set(cm, S.f4 & 0x000fffff);
   cm_set(cm, S.tt & 0x00000fff);
   h = S.w4 << 6;
@@ -371,13 +375,13 @@ P8_COLD P8_HD inline void sparse1_byte(State& S, int seenbefore, int howmany) { 
   cm_set(cm, (u64)(d + (h & 0xff000000)));
   cm_set(cm, S.w4 & 0xf0f0f0ff);
   cm_set(cm, (u64)((S.w4 & 63) * 128 + (5 << 17)));
-  cm_set(cm, (u64)((S.f4 & 0xffff) << 11 | S.frstchar));
-  cm_set(cm, (u64)(S.spafdo * 8 * ((S.w4 & 3) == 1)));
-  scm_set(M.scm[0], S.words & 127);
-  scm_set(M.scm[1], (S.words & 12) * 16 + (S.w4 & 12) * 4 + ((u32)buf(S, 1) >> 4));
+  cm_set(cm, (u64)((S.f4 & 0xffff) << 11 | W.frstchar));
+  cm_set(cm, (u64)(W.spafdo * 8 * ((S.w4 & 3) == 1)));
+  scm_set(M.scm[0], W.words & 127);
+  scm_set(M.scm[1], (W.words & 12) * 16 + (S.w4 & 12) * 4 + ((u32)buf(S, 1) >> 4));
   scm_set(M.scm[2], S.w4 & 15);
-  scm_set(M.scm[3], S.spafdo * ((S.w4 & 3) == 1));
-  scm_set(M.scm[6], S.frstchar);
+  scm_set(M.scm[3], W.spafdo * ((S.w4 & 3) == 1));
+  scm_set(M.scm[6], W.frstchar);
 }
 P8_COLD P8_HD inline void distance_byte(State& S) {   // :4598-4611
   DistanceM& M = S.distance;

@@ -912,7 +912,7 @@ P8_HD inline int context_model(State& S) {
   smatch_select(S);
   if (bpos == 0) { sparse_byte(S, ismatch, order); }
   cm_mix(S.sparse.cm, o, S.rnd, y, c0, bpos, buf(S, 1));
-  if (bpos == 0) sparse1_byte(S, ismatch, order);
+  if (bpos == 0) sparse1_byte(S, ismatch, order, word_stats(S));
   cm_mix(S.sparse1.cm, o, S.rnd, y, c0, bpos, buf(S, 1));
   for (int k = 0; k < 7; ++k) scm_mix(S.sparse1.scm[k], o, y);
   if (bpos == 0) distance_byte(S);

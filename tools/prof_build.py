@@ -15,6 +15,24 @@ CSRC = os.path.join(ROOT, "cmix_b200", "csrc")
 PROF_LIB = os.path.join(CSRC, "libcmixb200_prof.so")
 
 
+# PAQ8's slots. 0-11 add up to the model CTA's bit, 16-19 to the mixer CTA's. From 24 on: inside a byte the time a warp spent
+# in the probe (24 + warp) and apply (48 + warp) phases; on the bit that starts a byte the time, counted from the end of the
+# bookkeeping, at which a chain reached a point. The byte boundary's critical path is the latest of 24-30, 34-36 and 38,
+# which is what slot 2 waits for.
+P8_LABELS = {
+    0: "bookkeeping", 2: "byte boundary: until every chain is done (the join)", 3: "inside a byte: probe",
+    6: "byte boundary: probe of the 7-slot maps and the text history map", 7: "number (bits with a clash)", 8: "apply",
+    9: "selector sets, joining warp 12", 10: "waiting for a free ring slot", 11: "handing the bit over",
+    16: "mixer CTA: waiting for the model CTA", 17: "mixer CTA: SGD", 18: "mixer CTA: dot products", 19: "mixer CTA: final mixer, SSE",
+    24: "OLS 0 done | probe, warp 0", 25: "OLS 1 done | probe, warp 1", 26: "OLS 2 done | probe, warp 2", 27: "XML done | probe, warp 3",
+    28: "distance, record1 done | probe, warp 4", 29: "word chain done | probe, warp 5", 30: "nest, indirect done | probe, warp 6",
+    31: "D-chain: order-N and x86 contexts set | probe, warp 7", 32: "D-chain: history maps probed, match model | probe, warp 8",
+    33: "D-chain: history maps applied | probe, warp 9", 34: "D-chain: sparse done | probe, warp 10", 35: "D-chain: sparse1 done | probe, warp 11",
+    36: "D-chain: record done", 38: "text chain done",
+}
+P8_LABELS.update({48 + w: "apply, warp %d" % w for w in range(12)})
+
+
 def build():
     sys.path.insert(0, ROOT)
     from cmix_b200.capi import NVCC_COMPILE, NVCC_LINK
@@ -66,7 +84,7 @@ def run(n_bytes):
         print("%s: cycles per bit by phase (byte-boundary bits | other bits); clock %.0f MHz" % (name, sm_mhz))
         for k in range(rows):
             if a[0, k] or a[1, k]:
-                print("  phase %2d  %9.0f | %9.0f" % (k, a[0, k] / n_bytes, a[1, k] / (7 * n_bytes)))
+                print("  phase %2d  %9.0f | %9.0f   %s" % (k, a[0, k] / n_bytes, a[1, k] / (7 * n_bytes), P8_LABELS.get(k, "") if name == "paq8" else ""))
         # PAQ8 runs on two CTAs: the model CTA counts in slots 0-15 (10: waiting for a free ring slot), the mixer CTA in
         # 16-23 (16: waiting for a full slot); each CTA's total is its time per bit, less the mixer CTA's code-row writes
         parts = (("model CTA", 0, 16), ("mixer CTA", 16, 24)) if name == "paq8" else (("total", 0, 24),)
