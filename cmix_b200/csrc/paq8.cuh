@@ -11,8 +11,9 @@
 //    that draw; warp 0 numbers the flagged contexts in program order (ballot masks + a prefix over the maps) and produces the
 //    draws 24 at a time (the generator is a lagged XOR: x[i] = x[i-24] ^ x[i-55]); pass 2 applies them. A bit with a
 //    clashing map falls back to one lane walking the maps in order.
-//  * the match models, the DMC forest, the run maps and the direct maps run one unit per lane on warps 9-11 beside the
-//    context maps; on a bit inside a byte all of this is three phases (probe / number / apply). The bit that starts a byte
+//  * the match models, the DMC forest, the run maps and the direct maps run one unit per lane beside the context maps; on a
+//    bit inside a byte all of this is three phases (probe / number / apply), and the units take warps 9-11 and the text
+//    chain's idle warps 13-15, one function per warp and phase (lane map: P8_W_*). The bit that starts a byte
 //    first computes the new contexts, as chains of warps that do not wait for each other: the D-chain (order-N and x86
 //    contexts, their history maps, the match model, then the sparse and record models, which consume what the order-N map
 //    and the match model produce in the same bit), the word model, the text model with its stemmers, the three OLS
@@ -45,21 +46,40 @@ enum { P8_SEEN = 4096, P8_RING = 4 };
 // slots 0-11 the model CTA (2: from the end of the bookkeeping to the join of a byte boundary's chains, 10: waiting for a free
 // ring slot), 16-19 the mixer CTA (16: waiting for a full one). 24+: inside a byte the per-warp times of the probe (24 + warp)
 // and apply (48 + warp) phases; on a byte boundary the time from the end of the bookkeeping at which a chain got to a point
-// (24-30: warps 0-6 done, 31-36: the D-chain's steps, 38: the text chain done; labels in tools/prof_build.py)
+// (24-30: warps 0-6 done, 31-36: the D-chain's steps, 38: the text chain done). 64+: the longest lane of each single-lane
+// unit, from its own start to its end (P8_U). Labels in tools/prof_build.py.
+// Rows: 0 byte-boundary bits, 1 the others; the model CTA sums a bit in shared memory and also adds the bits inside a byte
+// by class into rows 2-5 (2 + 2 * "bpos 2 or 5: the 7-slot maps move to a new bucket" + "a 7-slot map clashes"). Slot
+// P8_PROF_N counts the model CTA's bits of a row.
 #ifdef P8_PROF
-__device__ unsigned long long g_p8_prof[2][96];
-#define P8_T(k) do { if (tid == 0) { const long long now_ = clock64(); atomicAdd(&g_p8_prof[sh.prof_row][k], (unsigned long long)(now_ - sh.prof_t)); sh.prof_t = now_; } } while (0)
+enum { P8_PROF_ROWS = 6, P8_PROF_SLOTS = 128, P8_PROF_UNIT = 64, P8_PROF_N = P8_PROF_SLOTS - 1 };
+__device__ unsigned long long g_p8_prof[P8_PROF_ROWS][P8_PROF_SLOTS];
+#define P8_T(k) do { if (tid == 0) { const long long now_ = clock64(); atomicAdd(&sh.prof_dst[k], (unsigned long long)(now_ - sh.prof_t)); sh.prof_t = now_; } } while (0)
 #define P8_M0 const long long m0_ = clock64()
-#define P8_M(slot) atomicAdd(&g_p8_prof[sh.prof_row][slot], (unsigned long long)(clock64() - m0_))
-#define P8_C(slot, n) atomicAdd(&g_p8_prof[sh.prof_row][slot], (unsigned long long)(n))
+#define P8_M(slot) atomicAdd(&sh.prof_dst[slot], (unsigned long long)(clock64() - m0_))
+#define P8_C(slot, n) atomicAdd(&sh.prof_dst[slot], (unsigned long long)(n))
+#define P8_U0 const long long u0_ = clock64()
+#define P8_U(g) atomicMax(&sh.prof_dst[P8_PROF_UNIT + (g)], (unsigned long long)(clock64() - u0_))
 #else
 #define P8_T(k) do { } while (0)
 #define P8_M0 do { } while (0)
 #define P8_M(slot) do { } while (0)
 #define P8_C(slot, n) do { } while (0)
+#define P8_U0 do { } while (0)
+#define P8_U(g) do { } while (0)
 #endif
 enum { P8_THREADS = 512, P8_WARPS = 16, P8_MAP_THREADS = 384, P8_MAP_WARPS = 12, P8_N_CM = 16, P8_N_CM2 = 3, P8_CM_LANES = 210, P8_CM2_LANES = 63, P8_N_UNITS = 53,
        P8_CM2_TID0 = 224, P8_TID_PIC = 287, P8_TID_MATCH = 288, P8_TID_W10 = 320, P8_TID_W11 = 352 };
+// Inside a byte warps 0-6 hold the 7-slot maps' lanes and warps 7-8 the history maps'; each of warps 9-11 and 13-15 runs one
+// function of the single-lane units per phase (lanes of one warp that diverge into different functions run one after another):
+//   probe   9 match_core   10 dmc_st x10   11 smatch_head   13 pic_core   14 record_pre   15 rcm_mix x3
+//   apply   9 imap_mix x3  10 pic_unit x3  11 DMC combination (and the constant input)
+//           13 sm32_p x5   14 scm_mix x18  15 stm_mix x13   (the maps behind the match, record, sparse match, sparse1 and
+//                                                             linear models, and the order-0/1 inputs)
+// warp 12 computes ModelStats and selector sets, as on every bit. Warps 13-15 skip the numbering of a clashing bit and the
+// barrier behind the maps' apply phase, so their apply overlaps both.
+enum { P8_W_MATCH = 9, P8_W_DMC = 10, P8_W_SMATCH = 11, P8_W_PIC = 13, P8_W_RECORD = 14, P8_W_RCM = 15,
+       P8_W_IMAP = 9, P8_W_PICU = 10, P8_W_DMCMIX = 11, P8_W_SM32 = 13, P8_W_SCM = 14, P8_W_STM = 15 };
 // Who computes the new contexts on the bit that starts a byte. A long single-lane job has a warp to itself while it runs
 // (lanes of one warp that diverge into different jobs run one after another):
 //   warps 0-2    the OLS predictors, lane 0 then the direct map behind its prediction
@@ -116,7 +136,8 @@ struct P8Shared {
     } mx;
   } u;
 #ifdef P8_PROF
-  long long prof_t; int prof_row;
+  long long prof_t; unsigned long long* prof_dst;   // the model CTA: prof_acc; the mixer CTA: its row of g_p8_prof
+  unsigned long long prof_acc[P8_PROF_SLOTS];
 #endif
 };
 
@@ -322,21 +343,19 @@ __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, i
   const u32 mask = __ballot_sync(0xffffffffu, flag);
   if ((tid & 31) == 0) sh.flag_mask[tid >> 5] = mask;
 }
-// the units that are one lane each (warps 8-11)
+// the units that are one lane each, on the bit that starts a byte (warps 8-11 of the D-chain; record_pre and the linear
+// predictions' maps follow their models there)
 __device__ __noinline__ void p8_probe_single(P8Shared& sh, int tid, int y, int c0, int bpos) {
   using namespace p8;
   State& S = sh.S;
   const p8::Tables& T = *S.T;
   if (tid == P8_TID_PIC) pic_core(S);
   else if (tid == P8_TID_MATCH) { Out o = p8_out(sh, sh.unit_off[7]); match_core(S, o); }
-  else if (tid == P8_TID_MATCH + 1) { if (bpos != 0) record_pre(S); }   // on a byte boundary it follows record_byte
   else if (tid >= P8_TID_W10 && tid < P8_TID_W10 + 10) sh.dmc_st[tid - P8_TID_W10] = dmc_st(T, S.dmc[tid - P8_TID_W10], y);
   else if (tid >= P8_TID_MATCH + 2 && tid < P8_TID_MATCH + 5) {
     const int r = tid - (P8_TID_MATCH + 2);
     Out o = p8_out(sh, sh.unit_off[4 + r]);
     rcm_mix(r == 0 ? S.rcm7 : r == 1 ? S.rcm9 : S.rcm10, o, c0, bpos);
-  } else if (tid >= P8_TID_W11 + 4 && tid < P8_TID_W11 + 9) {   // on a byte boundary each follows its predictor
-    if (bpos != 0) { const int r = tid - (P8_TID_W11 + 4); Out o = p8_out(sh, sh.unit_off[48 + r]); linear_small(S, o, r); }
   }
   else if (tid == P8_TID_W11) { Out o = p8_out(sh, sh.unit_off[8]); smatch_head(S, o); }
   else if (tid == P8_TID_W11 + 1 || tid == P8_TID_W11 + 2) {
@@ -418,6 +437,19 @@ __device__ __noinline__ void p8_apply_cm(P8Shared& sh, int tid, int y, int c0, i
   Out o = p8_out(sh, sh.unit_off[c_p8_cm_unit[k]] + 5 * i);
   cm_step(m, i, o, ns, y, c0, bpos, buf(sh.S, 1));
 }
+// DMC forest combination, and the reset at a byte boundary (dmcForest::mix), from the dmc_st values of the probe
+__device__ __forceinline__ void p8_dmc_mix(P8Shared& sh, p8::Out& o, int bpos) {
+  using namespace p8;
+  State& S = sh.S;
+  const u32 params[10] = {2, 32, 64, 4, 128, 8, 256, 16, 1024, 1536};
+  add(o, sh.dmc_st[9] >> 3);
+  add(o, sh.dmc_st[8] >> 3);
+  for (int i = 7; i > 0; i -= 2) add(o, (sh.dmc_st[i] + sh.dmc_st[i - 1]) >> 4);
+  if (bpos == 0)
+    for (int i = 7; i >= 0; --i)
+      if ((S.dmc[i].extra >> 7) > S.dmc[i].size) dmc_reset(S.dmc[i], params[i]);
+}
+// the units that are one lane each, on the bit that starts a byte (warps 9-11 after the join)
 __device__ __noinline__ void p8_apply_small(P8Shared& sh, int tid, int y, int bpos) {
   using namespace p8;
   State& S = sh.S;
@@ -429,13 +461,7 @@ __device__ __noinline__ void p8_apply_small(P8Shared& sh, int tid, int y, int bp
     record_small(S, o, tid - P8_TID_W10);
   } else if (tid == P8_TID_W10 + 12) {                     // DMC forest combination and reset (dmcForest::mix)
     Out o = p8_out(sh, sh.unit_off[44]);
-    const u32 params[10] = {2, 32, 64, 4, 128, 8, 256, 16, 1024, 1536};
-    add(o, sh.dmc_st[9] >> 3);
-    add(o, sh.dmc_st[8] >> 3);
-    for (int i = 7; i > 0; i -= 2) add(o, (sh.dmc_st[i] + sh.dmc_st[i - 1]) >> 4);
-    if (bpos == 0)
-      for (int i = 7; i >= 0; --i)
-        if ((S.dmc[i].extra >> 7) > S.dmc[i].size) dmc_reset(S.dmc[i], params[i]);
+    p8_dmc_mix(sh, o, bpos);
   } else if (tid >= P8_TID_W11 && tid < P8_TID_W11 + 7) {   // sparseModel1's seven stationary maps
     Out o = p8_out(sh, sh.unit_off[11 + (tid - P8_TID_W11)]);
     scm_mix(S.sparse1.scm[tid - P8_TID_W11], o, y);
@@ -445,6 +471,76 @@ __device__ __noinline__ void p8_apply_small(P8Shared& sh, int tid, int y, int bp
   } else if (tid >= P8_TID_W11 + 11 && tid < P8_TID_W11 + 14) {
     Out o = p8_out(sh, sh.unit_off[19]);
     pic_unit(S, o, tid - (P8_TID_W11 + 11));
+  }
+}
+
+// ---- inside a byte: the single-lane units, a warp per function (lane map: P8_W_* below). Every unit writes its inputs at
+// its own unit_off[] as on the bit that starts a byte; units of one phase share no state, so their order does not matter.
+__device__ __noinline__ void p8_probe_units(P8Shared& sh, int warp, int lane, int y, int c0, int bpos) {
+  using namespace p8;
+  State& S = sh.S;
+  P8_U0;
+  if (warp == P8_W_MATCH) {
+    if (lane == 0) { Out o = p8_out(sh, sh.unit_off[7]); match_core(S, o); P8_U(1); }
+  } else if (warp == P8_W_DMC) {
+    if (lane < 10) { sh.dmc_st[lane] = dmc_st(*S.T, S.dmc[lane], y); P8_U(4); }
+  } else if (warp == P8_W_SMATCH) {
+    if (lane == 0) { Out o = p8_out(sh, sh.unit_off[8]); smatch_head(S, o); P8_U(5); }
+  } else if (warp == P8_W_PIC) {
+    if (lane == 0) { pic_core(S); P8_U(0); }
+  } else if (warp == P8_W_RECORD) {
+    if (lane == 0) { record_pre(S); P8_U(2); }
+  } else if (warp == P8_W_RCM) {
+    if (lane < 3) { Out o = p8_out(sh, sh.unit_off[4 + lane]); rcm_mix(lane == 0 ? S.rcm7 : lane == 1 ? S.rcm9 : S.rcm10, o, c0, bpos); P8_U(3); }
+  }
+}
+// The apply phase groups the units by the map they end in, so that the lanes of a warp run one call of one function with
+// their own arguments (the arguments are those of match_unit, record_small, smatch_unit, linear_small and the rest).
+__device__ __noinline__ void p8_apply_units(P8Shared& sh, int warp, int lane, int y, int c0, int bpos) {
+  using namespace p8;
+  State& S = sh.S;
+  const p8::Tables& T = *S.T;
+  P8_U0;
+  if (warp == P8_W_SM32) {              // the match model's three StateMaps (match_unit 0-2), the order-0 and order-1 inputs
+    if (lane >= 5) return;
+    Sm32* s; int off, cx; bool on = true;
+    if (lane < 3) { s = &S.match.sm[lane]; off = sh.unit_off[7] + 2 + lane; cx = (int)S.match.ctx[lane]; on = cx != 0; }
+    else { s = lane == 3 ? &S.sm0 : &S.sm1; off = sh.unit_off[lane - 2]; cx = lane == 3 ? c0 : (c0 | (buf(S, 1) << 8)); }
+    Out o = p8_out(sh, off);
+    const int p = sm32_p(T, *s, y, cx);
+    add(o, on ? (stretch(T, p) + 1) >> 1 : 0);
+    P8_U(10);
+  } else if (warp == P8_W_SCM) {        // match_unit 3-5, record_small 9-11, sparseModel1's seven maps, linear_small 0-4
+    if (lane >= 18) return;
+    Scm* c; int off, rate = 7, mul = 1, div = 4;
+    if (lane < 3) { c = &S.match.scm[lane]; off = sh.unit_off[7] + 5 + 2 * lane; rate = 7 - lane; }
+    else if (lane < 6) { const int k = lane - 3; c = &S.record.smap[k]; off = sh.unit_off[33 + k]; rate = k < 2 ? 6 : 5; div = k < 2 ? 3 : 2; }
+    else if (lane < 13) { c = &S.sparse1.scm[lane - 6]; off = sh.unit_off[11 + lane - 6]; }
+    else {
+      const int i = lane - 13;
+      LinearM& M = S.linear;
+      c = &M.smap[i]; off = sh.unit_off[48 + i]; rate = 6; div = 2;
+      scm_set(*c, (u32)((M.prd[i] - (u8)(c0 << (8 - bpos))) * 8 + bpos));
+    }
+    Out o = p8_out(sh, off);
+    scm_mix(*c, o, y, rate, mul, div);
+    P8_U(11);
+  } else if (warp == P8_W_STM) {        // match_unit 6-8, record_small 0-5, smatch_unit 0-3
+    if (lane >= 13 || (lane >= 9 && !S.smatch.valid)) return;
+    Stm* c; int off, div = 4, limit = 1023;
+    if (lane < 3) { c = &S.match.maps[lane]; off = sh.unit_off[7] + 11 + 2 * lane; limit = lane == 0 ? 255 : 1023; }
+    else if (lane < 9) { c = &S.record.maps[lane - 3]; off = sh.unit_off[24 + lane - 3]; div = 3; }
+    else { c = &S.smatch.maps[lane - 9]; off = sh.unit_off[8] + 3 + 2 * (lane - 9); div = 2; }
+    Out o = p8_out(sh, off);
+    stm_mix(*c, o, y, 1, div, limit);
+    P8_U(12);
+  } else if (warp == P8_W_IMAP) {       // record_small 6-8
+    if (lane < 3) { Out o = p8_out(sh, sh.unit_off[30 + lane]); imap_mix(S.record.imap[lane], o, y, 1, 3, 255); P8_U(13); }
+  } else if (warp == P8_W_PICU) {
+    if (lane < 3) { Out o = p8_out(sh, sh.unit_off[19]); pic_unit(S, o, lane); P8_U(17); }
+  } else if (warp == P8_W_DMCMIX) {     // the DMC forest's combination (from dmc_st of the probe) and the constant input
+    if (lane == 0) { Out o = p8_out(sh, sh.unit_off[44]); p8_dmc_mix(sh, o, bpos); P8_U(14); }
+    else if (lane == 1) { Out o = p8_out(sh, sh.unit_off[0]); add(o, 64); }
   }
 }
 
@@ -526,6 +622,9 @@ static_assert(p8::N_IN % 8 == 0 && p8::N_IN / 8 <= 7 * 32, "a weight row is at m
 // first SGD warp waits for it (sync) and computes those sets beside the apply phase
 __device__ __forceinline__ void p8_signal_selects() { asm volatile("bar.arrive 2, 416;" ::: "memory"); }
 __device__ __forceinline__ void p8_await_selects() { asm volatile("bar.sync 2, 416;" ::: "memory"); }
+// named barrier 1 (warps 0-11): behind lane 0's numbering of a clashing bit and behind the apply phase, before lane 0's
+// epilogue reads res2 and clash; on the bit that starts a byte also between the probe and the numbering. Inside a byte the
+// unit warps 13-15 are not in it (nothing behind it reads their inputs before the bit's last __syncthreads)
 __device__ __forceinline__ void p8_sync_maps() { asm volatile("bar.sync 1, 384;" ::: "memory"); static_assert(P8_MAP_THREADS == 384, "named barrier width"); }
 // The bit that starts a byte runs its context computation as independent chains of warps (p8_model_bit) ordered by three
 // more named barriers. Every arrive / sync below is executed by whole warps, unconditionally on that bit:
@@ -533,6 +632,8 @@ __device__ __forceinline__ void p8_sync_maps() { asm volatile("bar.sync 1, 384;"
 //                 (384), the text chain's warps 13-15 arrive (96) and go on to the end of the bit.
 //  4 (160):       the D-chain's warps 7-11 between its steps.
 //  5 (96):        the text chain's warps 13-15 between its steps.
+// Inside a byte barrier 3 is the probe / apply boundary, with the same warps: all of them sync (the unit warps 13-15 apply
+// what warps 9-11 probed and the reverse).
 __device__ __forceinline__ void p8_join_sync() { asm volatile("bar.sync 3, 480;" ::: "memory"); }
 __device__ __forceinline__ void p8_join_arrive() { __threadfence_block(); asm volatile("bar.arrive 3, 480;" ::: "memory"); }
 __device__ __forceinline__ void p8_sync_dchain() { asm volatile("bar.sync 4, 160;" ::: "memory"); }
@@ -541,6 +642,9 @@ enum { P8_WARP_D = P8_CM2_TID0 / 32, P8_WARP_TEXT = P8_MAP_WARPS + 1 };   // fir
 static_assert(P8_CM2_TID0 % 32 == 0 && P8_CM_LANES <= P8_CM2_TID0 && (P8_MAP_WARPS - P8_WARP_D) * 32 == 160, "barrier 4: warps 7-11");
 static_assert((P8_WARPS - P8_WARP_TEXT) * 32 == 96 && P8_MAP_THREADS + 96 == 480, "barriers 3 and 5: warps 13-15 beside the 12 map warps");
 static_assert(P8_TID_MATCH == (P8_WARP_D + 2) * 32 && P8_TID_W10 == (P8_WARP_D + 3) * 32 && P8_TID_W11 == (P8_WARP_D + 4) * 32, "a warp per long job of the D-chain");
+static_assert(P8_W_MATCH > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_SMATCH < (int)P8_MAP_WARPS && (int)P8_W_PIC == (int)P8_WARP_TEXT && (int)P8_W_RCM == (int)P8_WARPS - 1 &&
+              P8_W_IMAP > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_DMCMIX < (int)P8_MAP_WARPS && (int)P8_W_SM32 == (int)P8_WARP_TEXT && (int)P8_W_STM == (int)P8_WARPS - 1,
+              "barrier 3 inside a byte: the unit warps are 9-11 (in barriers 1 and 2 with the map warps) and 13-15 (in barrier 3 only)");
 
 // The ring's mbarriers. An arrive on the other CTA's barrier releases at cluster scope what the arriving thread wrote or
 // read before it; a wait acquires it.
@@ -593,13 +697,17 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
   const p8::Tables& T = *S.T;
   const int warp = tid >> 5, lane = tid & 31;
 #ifdef P8_PROF
-  if (tid == 0) { sh.prof_t = clock64(); sh.prof_row = (S.bpos == 7) ? 0 : 1; }   // bpos before bit_begin: 7 -> this bit starts a byte
+  if (tid == 0) { sh.prof_t = clock64(); sh.prof_dst = sh.prof_acc; }
+  int prof_clash = 0;   // lane 0: any_clash as the bit ends (the next bit's bookkeeping resets it beside the handover)
 #endif
   // ---- phase 0: bookkeeping (bit_begin's st_misses line works on a stale S.pr here: st_misses belongs to the mixer CTA)
   if (tid == 0) {
+    P8_U0;
     bit_begin(S, y);
     if (S.bpos == 0) block_parse(S);
-    sh.snap = word_stats(S);
+    P8_U(20);
+    if (S.bpos == 0) sh.snap = word_stats(S);     // read by sparse1_byte only
+    P8_U(21);
   }
   if (tid >= 32 && tid < 32 + P8_N_CM) sh.clash[tid - 32] = 0;
   if (tid >= 64 && tid < 64 + P8_N_CM2) { sh.clash2[tid - 64] = 0; sh.res2[tid - 64] = 0; }
@@ -620,7 +728,11 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     sh.unit_off[lane] = ia - a;
     if (lane + 32 <= P8_N_UNITS) sh.unit_off[lane + 32] = ta + ib - b;
   }
-  for (int k = tid; k < P8_SEEN; k += P8_THREADS) sh.u.md.seen[k] = 0ull;
+  {
+    P8_U0;
+    for (int k = tid; k < P8_SEEN; k += P8_THREADS) sh.u.md.seen[k] = 0ull;
+    if (tid == 0) P8_U(22);
+  }
   __syncthreads();
   P8_T(0);
   const int bpos = S.bpos, c0 = S.c0;
@@ -661,6 +773,21 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         if (lane == 0) { S.text.map.index = n; P8_M(38); }
       }
       p8_join_arrive();
+    } else {
+      // ---- inside a byte, warps 13-15: single-lane units beside the maps; the apply runs while lane 0 numbers a clashing bit
+      {
+        P8_M0;
+        p8_probe_units(sh, warp, lane, y, c0, bpos);
+        __syncwarp();
+        if (lane == 0) P8_M(24 + warp);
+      }
+      p8_join_sync();
+      {
+        P8_M0;
+        p8_apply_units(sh, warp, lane, y, c0, bpos);
+        __syncwarp();
+        if (lane == 0) P8_M(48 + warp);
+      }
     }
   } else {
     if (tid == 0) { S.m.nx = S.m.base = S.m.ncxt = 0; }
@@ -726,15 +853,17 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       p8_sync_maps();
       P8_T(8);
     } else {
-      // ---- inside a byte: probe / number / apply, all map families side by side
+      // ---- inside a byte: probe / number / apply, all map families side by side, the single-lane units on warps 9-11 and
+      // 13-15 (lane map: P8_W_*)
       {
         P8_M0;
         if (warp < 7) p8_probe_cm(sh, tid, y, c0, bpos);
-        else { p8_probe_cm2(sh, tid, bpos, 7); p8_probe_single(sh, tid, y, c0, bpos); }
+        else if (warp < P8_W_MATCH) p8_probe_cm2(sh, tid, bpos, 7);
+        else p8_probe_units(sh, warp, lane, y, c0, bpos);
         __syncwarp();
         if (lane == 0) P8_M(24 + warp);
       }
-      p8_sync_maps();
+      p8_join_sync();
       p8_signal_selects();
       P8_T(3);
       if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(); }
@@ -742,7 +871,8 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       {
         P8_M0;
         if (warp < 7) p8_apply_cm(sh, tid, y, c0, bpos);
-        else { p8_apply_cm2(sh, tid, y, bpos, 7); p8_apply_small(sh, tid, y, bpos); }
+        else if (warp < P8_W_IMAP) p8_apply_cm2(sh, tid, y, bpos, 7);
+        else p8_apply_units(sh, warp, lane, y, c0, bpos);
         __syncwarp();
         if (lane == 0) P8_M(48 + warp);
       }
@@ -751,6 +881,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     }
     // ---- epilogues, ModelStats, the 28 selector sets in the reference's order
     if (tid == 0) {
+      P8_U0;
       if (bpos == 7) {
         for (int k = 0; k < P8_N_CM; ++k) if (!sh.clash[k]) p8_cm(S, k).cn = 0;
         for (int k = 0; k < P8_N_CM2; ++k) p8_cm2(S, k).index = 0;
@@ -760,6 +891,10 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       m.nx = sh.unit_off[P8_N_UNITS];
       m.n2 = m.nx;
       while (m.nx & 7) m.tx[m.nx++] = 0;
+      P8_U(23);
+#ifdef P8_PROF
+      prof_clash = sh.any_clash != 0;
+#endif
     }
   }
   __syncthreads();     // warp 12 joins
@@ -786,6 +921,18 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     if (lane == 0) p8_mbar_arrive_remote(&sh.full[slot], 1);
   }
   P8_T(11);
+#ifdef P8_PROF
+  // the other lanes record nothing before the next bit's first barrier, which lane 0 reaches after this
+  if (tid == 0) {
+    const int row = S.bpos == 0 ? 0 : 2 + 2 * (S.bpos == 2 || S.bpos == 5) + prof_clash;
+    sh.prof_acc[P8_PROF_N] = 1;
+    for (int k = 0; k < P8_PROF_SLOTS; ++k) {
+      atomicAdd(&g_p8_prof[row ? 1 : 0][k], sh.prof_acc[k]);
+      if (row) atomicAdd(&g_p8_prof[row][k], sh.prof_acc[k]);
+      sh.prof_acc[k] = 0;
+    }
+  }
+#endif
 }
 static_assert(offsetof(p8::State, codes) % 4 == 0 && p8::N_IN % 2 == 0, "codes are handed over in 4-byte words");
 
@@ -802,7 +949,7 @@ __device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_p
   const int slot = (int)(t % P8_RING);
   const P8Slot& in = sh.u.mx.ring[slot];
 #ifdef P8_PROF
-  if (tid == 0) { sh.prof_t = clock64(); sh.prof_row = nb == 0 ? 0 : 1; }
+  if (tid == 0) { sh.prof_t = clock64(); sh.prof_dst = g_p8_prof[nb == 0 ? 0 : 1]; }
 #endif
   // ---- SGD of the previous bit's sets and of the final mixer
   p8_sgd(sh, tx_prev, y, tid);
@@ -887,6 +1034,9 @@ __device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g
   const p8::Tables* gT = sh.S.T;
   p8_copy_words(sh.tab, gT, p8::TABLES_HOT_BYTES, tid);
   if (tid < p8::N_SETS) sh.wc_set[tid] = -1;
+#ifdef P8_PROF
+  for (int k = tid; k < P8_PROF_SLOTS; k += P8_THREADS) sh.prof_acc[k] = 0;
+#endif
   if (tid == 0) {
     for (int i = 0; i < P8_RING; ++i) {
       if (rank == 0) p8_mbar_init(&sh.empty[i], 1);

@@ -22,7 +22,7 @@ void paq8_launch_bit(p8::State* g, int y, u16* ext_bit, cudaStream_t s, const u3
 extern "C" int cmixb200_p8_prof(unsigned long long* out, int reset) {
   cudaDeviceSynchronize();
   if (cudaMemcpyFromSymbol(out, cmixb200::g_p8_prof, sizeof(cmixb200::g_p8_prof)) != cudaSuccess) return 1;
-  if (reset) { static unsigned long long z[2][96]; cudaMemcpyToSymbol(cmixb200::g_p8_prof, z, sizeof(z)); }
+  if (reset) { static unsigned long long z[cmixb200::P8_PROF_ROWS][cmixb200::P8_PROF_SLOTS]; cudaMemcpyToSymbol(cmixb200::g_p8_prof, z, sizeof(z)); }
   return 0;
 }
 #endif

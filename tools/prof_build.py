@@ -30,7 +30,38 @@ P8_LABELS = {
     33: "D-chain: history maps applied | probe, warp 9", 34: "D-chain: sparse done | probe, warp 10", 35: "D-chain: sparse1 done | probe, warp 11",
     36: "D-chain: record done", 38: "text chain done",
 }
-P8_LABELS.update({48 + w: "apply, warp %d" % w for w in range(12)})
+P8_LABELS.update({48 + w: "apply, warp %d" % w for w in range(16)})
+for w in range(13, 16):
+    P8_LABELS[24 + w] = (P8_LABELS[24 + w] + " | " if 24 + w in P8_LABELS else "") + "probe, warp %d" % w
+# 64 + g: single-lane unit g, the time from its warp's entry into the phase's unit code to the end of the unit (the latest
+# lane; where a warp's lanes diverge into several units this includes the units that ran before it). Inside a byte only.
+P8_UNITS = {
+    0: "probe: pic_core", 1: "probe: match_core", 2: "probe: record_pre", 3: "probe: rcm_mix x3", 4: "probe: dmc_st x10",
+    5: "probe: smatch_head",
+    10: "apply: sm32_p x5 (match x3, order 0-1 x2)", 11: "apply: scm_mix x18 (match, record, sparse1, linear)",
+    12: "apply: stm_mix x13 (match, record, sparse match)", 13: "apply: imap_mix x3 (record)", 14: "apply: DMC combination, add(64)",
+    17: "apply: pic_unit x3",
+    20: "lane 0: bit_begin, block_parse", 21: "lane 0: word_stats snapshot", 22: "lane 0: its share of clearing `seen`",
+    23: "lane 0: epilogue (main_select_fixed, padding)",
+}
+P8_LABELS.update({64 + g: "unit: " + s for g, s in P8_UNITS.items()})
+P8_ROWS, P8_SLOTS = 6, 128
+P8_CLASSES = ["byte boundary", "inside a byte", "same bucket", "same bucket, clash", "new bucket", "new bucket, clash"]
+
+
+P8_PROF_N = P8_SLOTS - 1   # the model CTA's bits in a row
+
+
+def paq8_classes(a):
+    """The model CTA's cycles per bit by phase and unit, one column per class of bit (row 1 = rows 2-5)."""
+    n = a[:, P8_PROF_N]
+    cols = [r for r in range(P8_ROWS) if n[r]]
+    print("paq8 model CTA: cycles per bit by class of bit (bits: %s)" % ", ".join("%s %d" % (P8_CLASSES[r], n[r]) for r in cols))
+    print("  %-5s " % "slot" + "".join("%19s" % P8_CLASSES[r] for r in cols))
+    for k in list(range(16)) + list(range(24, P8_PROF_N)):
+        if any(a[r, k] for r in cols):
+            print("  %-5d " % k + "".join("%19.0f" % (a[r, k] / n[r]) for r in cols) + "   " + P8_LABELS.get(k, ""))
+    print("  %-5s " % "total" + "".join("%19.0f" % (a[r, :16].sum() / n[r]) for r in cols))
 
 
 def build():
@@ -48,7 +79,7 @@ def build():
 
 
 def run(n_bytes):
-    os.environ["CMIXB200_LIB"] = PROF_LIB
+    os.environ.setdefault("CMIXB200_LIB", PROF_LIB)   # or another profiling build, to compare two
     sys.path.insert(0, ROOT)
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import numpy as np
@@ -63,26 +94,30 @@ def run(n_bytes):
     P.code_bytes(text[:n_bytes])
     lib = load_library()
     sm_mhz = torch.cuda.get_device_properties(0).clock_rate / 1e3 if hasattr(torch.cuda.get_device_properties(0), "clock_rate") else 1980.0
-    for name, fn, rows in (("paq8", "cmixb200_p8_prof", 96), ("fxcm", "cmixb200_fx_prof", 24)):
+    for name, fn, size in (("paq8", "cmixb200_p8_prof", P8_ROWS * P8_SLOTS), ("fxcm", "cmixb200_fx_prof", 2 * 24)):
         if not hasattr(lib, fn):
             continue
-        buf = (ctypes.c_ulonglong * (2 * rows))()
+        buf = (ctypes.c_ulonglong * size)()
         getattr(lib, fn)(buf, 1)
     P.time_mix_kernel(True)
     P.code_bytes(text[n_bytes:2 * n_bytes])
     for w, k in enumerate(["mix", "small", "lstm", "ppmd", "fxcm", "paq8"]):
         ms, n = P.kernel_ms(w)
         print("%-6s %8.2f us/bit (%d launches)" % (k, ms * 1e3 / (n_bytes * 8), n))
-    for name, fn, rows in (("paq8", "cmixb200_p8_prof", 96), ("fxcm", "cmixb200_fx_prof", 24)):
+    for name, fn, rows in (("paq8", "cmixb200_p8_prof", P8_SLOTS), ("fxcm", "cmixb200_fx_prof", 24)):
         try:
             f = getattr(lib, fn)
         except AttributeError:
             continue
-        buf = (ctypes.c_ulonglong * (2 * rows))()
+        n_rows = P8_ROWS if name == "paq8" else 2
+        buf = (ctypes.c_ulonglong * (n_rows * rows))()
         f(buf, 0)
-        a = np.array(list(buf), dtype=np.float64).reshape(2, rows)
+        a = np.array(list(buf), dtype=np.float64).reshape(n_rows, rows)
+        if name == "paq8":
+            paq8_classes(a)
+            a = a[:2, :P8_PROF_N]
         print("%s: cycles per bit by phase (byte-boundary bits | other bits); clock %.0f MHz" % (name, sm_mhz))
-        for k in range(rows):
+        for k in range(a.shape[1]):
             if a[0, k] or a[1, k]:
                 print("  phase %2d  %9.0f | %9.0f   %s" % (k, a[0, k] / n_bytes, a[1, k] / (7 * n_bytes), P8_LABELS.get(k, "") if name == "paq8" else ""))
         # PAQ8 runs on two CTAs: the model CTA counts in slots 0-15 (10: waiting for a free ring slot), the mixer CTA in
