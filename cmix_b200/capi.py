@@ -13,7 +13,7 @@ import numpy as np
 N_EXT = 2022
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
-LIB_PATH = os.environ.get("CMIXB200_LIB") or os.path.join(CSRC, "libcmixb200.so")   # CMIXB200_LIB: a profiling build (tools/prof_build.py)
+LIB_PATH = os.environ.get("CMIXB200_LIB") or os.path.join(CSRC, "libcmixb200.so")   # CMIXB200_LIB: a profiling (tools/prof_build.py) or jitter (tests/test_schedule_jitter.py) build
 NVCC_COMPILE = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 NVCC_LINK = ["-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC"]
 NVCC_FLAGS = NVCC_COMPILE + ["-shared"]

@@ -8,6 +8,7 @@
 #ifndef CMIXB200_CODER_CUH
 #define CMIXB200_CODER_CUH
 #include "exact_math.h"
+#include "jitter.cuh"
 #include "state.h"
 
 namespace cmixb200 {
@@ -21,7 +22,7 @@ __device__ __forceinline__ void coder_shift_out(CoderState& c) {
   }
 }
 
-__global__ void __launch_bounds__(32, 1) encode_kernel(const ChunkArgs* __restrict__ args) {
+__global__ void __launch_bounds__(32, 1) encode_kernel(const ChunkArgs* __restrict__ args) { jit_entry(JK_ENCODE);
   const ChunkArgs a = args[blockIdx.x];
   if (a.coder == nullptr || threadIdx.x != 0) return;
   CoderState c = *a.coder;
@@ -37,7 +38,7 @@ __global__ void __launch_bounds__(32, 1) encode_kernel(const ChunkArgs* __restri
   *a.coder = c;
 }
 
-__global__ void encode_flush_kernel(CoderState* cs) {                 // Encoder::Flush, encoder.cpp:32-39
+__global__ void encode_flush_kernel(CoderState* cs) { jit_entry(JK_ENCODE_FLUSH);                 // Encoder::Flush, encoder.cpp:32-39
   CoderState c = *cs;
   coder_shift_out(c);
   if (c.n_out < c.cap) c.out[c.n_out] = (u8)(c.x2 >> 24); else c.overflow = 1;
@@ -48,13 +49,13 @@ __global__ void encode_flush_kernel(CoderState* cs) {                 // Encoder
 // One step of Decoder::Decode (reference src/coder/decoder.cpp:16-39) between the predict and the perceive kernels of a bit, on
 // the device: the probability never leaves HBM and the decoded bit is handed to the perceive kernels through DecodeState.
 __device__ __forceinline__ u32 decoder_read_byte(DecodeState& d) { return d.pos < d.n_arch ? d.arch[d.pos++] : 0u; }   // decoder.cpp:10-14
-__global__ void decode_begin_kernel(DecodeState* ds) {                // Decoder::Decoder, decoder.cpp:3-8
+__global__ void decode_begin_kernel(DecodeState* ds) { jit_entry(JK_DECODE_BEGIN);                // Decoder::Decoder, decoder.cpp:3-8
   DecodeState d = *ds;
   d.x1 = 0; d.x2 = 0xffffffffu; d.x = 0; d.ctx = 1; d.t = 0; d.bit = d.full = 0;
   for (int i = 0; i < 4; ++i) d.x = (d.x << 8) + (decoder_read_byte(d) & 0xff);
   *ds = d;
 }
-__global__ void decode_step_kernel(const StreamState* st, DecodeState* ds) {
+__global__ void decode_step_kernel(const StreamState* st, DecodeState* ds) { jit_entry(JK_DECODE_STEP);
   DecodeState d = *ds;
   const u32 p = (u32)XM_FADD(1.0f, XM_FMUL(65534.0f, st->last_p));   // Decoder::Discretize, decoder.cpp:16-18
   const u32 range = d.x2 - d.x1;

@@ -28,6 +28,7 @@
 
 #include "../../include/cmixb200.h"
 #include "exact_math.h"
+#include "jitter.cuh"
 #include "coder.cuh"
 #include "fxcm_model.h"
 #include "fxcm_host.h"
@@ -141,13 +142,13 @@ struct GlibcRand {   // the rand() stream of one Predictor (TYPE_3 additive feed
   int next() { int32_t r; random_r(&rd, &r); return r; }
 };
 
-__global__ void fill_f32(float* p, size_t n, float v) {
+__global__ void fill_f32(float* p, size_t n, float v) { jit_entry(JK_FILL);
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
-__global__ void fill_u32(u32* p, size_t n, u32 v) {
+__global__ void fill_u32(u32* p, size_t n, u32 v) { jit_entry(JK_FILL);
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
-__global__ void fill_sse_rows(u16* p, size_t vol, int Wi) {   // SSEi<7>::Init (sse.cpp:25-31), 8-u16 pitch
+__global__ void fill_sse_rows(u16* p, size_t vol, int Wi) { jit_entry(JK_FILL);   // SSEi<7>::Init (sse.cpp:25-31), 8-u16 pitch
   const int SCw = (32768 - Wi) / 6, INC = Wi / 2 + 8192;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < vol * 8; i += (size_t)gridDim.x * blockDim.x) {
     const int k = (int)(i & 7);
@@ -360,7 +361,7 @@ int InitDirect(cmixb200_predictor* P, DirectTable& d, int limit, float delta, u6
   return CMIXB200_OK;
 }
 
-__global__ void fill_u16(u16* p, size_t n, u16 v) {
+__global__ void fill_u16(u16* p, size_t n, u16 v) { jit_entry(JK_FILL);
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
 // Memory backend of fx::build_state (fxcm_host.h): zeroed cudaMalloc, fill kernels, blocking uploads.
@@ -1321,3 +1322,26 @@ int cmixb200_debug_fetch(cmixb200_predictor* P, int what, void* out, size_t byte
 }
 
 }  // extern "C"
+
+#ifdef CMIXB200_JITTER
+// Jitter build only (jitter.cuh): the schedule of every kernel's sleeps, and per site how often a sleep ran. Not in
+// include/cmixb200.h: a product build does not have them.
+namespace cmixb200 { JIT_MODULE(engine) }
+extern "C" int cmixb200_jitter_config(int mode, unsigned seed, int a, int b, int c) {
+  for (auto set : {jit_set_engine, jit_set_fxcm, jit_set_paq8}) {
+    const cudaError_t e = set(mode, seed, a, b, c);
+    if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return CMIXB200_ERR_CUDA; }
+  }
+  return CMIXB200_OK;
+}
+// out: JIT_N_FILES * JIT_MAX_LINE counts, site = file * JIT_MAX_LINE + line (files in JIT_FILE_LIST's order)
+extern "C" int cmixb200_jitter_counts(unsigned* out, size_t n) {
+  if (n != (size_t)JIT_N_FILES * JIT_MAX_LINE) { g_last_error = "jitter counts: wrong size"; return CMIXB200_ERR_ARG; }
+  memset(out, 0, n * sizeof *out);
+  for (auto get : {jit_fired_engine, jit_fired_fxcm, jit_fired_paq8}) {
+    const cudaError_t e = get(out);
+    if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return CMIXB200_ERR_CUDA; }
+  }
+  return CMIXB200_OK;
+}
+#endif

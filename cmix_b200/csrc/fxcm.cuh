@@ -15,6 +15,7 @@
 // memory for the launch; the per-map tables and the ~4.6 GB of model memory stay in HBM.
 #pragma once
 #include "exact_math.h"
+#include "jitter.cuh"
 #include "fxcm_model.h"
 #include "bytemodel.cuh"
 #include "state.h"
@@ -70,7 +71,7 @@ __device__ __forceinline__ FxGlobals fx_load(FxShared& sh, fx::State* g, int tid
   fx_copy_words(&sh.S, g, sizeof(fx::State), tid);
   fx_copy_words(&sh.X, r.gx, sizeof(fx::TextState), tid);
   fx_copy_words(sh.tab, r.gT, fx::TABLES_HOT_BYTES, tid);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) { sh.S.text = &sh.X; sh.S.T = reinterpret_cast<const fx::Tables*>(sh.tab); }
   const int warp = tid >> 5, lane = tid & 31;
   if (warp < 10) {
@@ -78,15 +79,15 @@ __device__ __forceinline__ FxGlobals fx_load(FxShared& sh, fx::State* g, int tid
     fx_row_load(sh.w1[warp], m.w + (size_t)m.cxt * fx::N_IN1, lane);
     if (lane == 0) sh.w_set[warp] = m.cxt;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   return r;
 }
 __device__ __forceinline__ void fx_store(FxShared& sh, fx::State* g, const FxGlobals& r, int tid) {
-  __syncthreads();
+  JIT_SYNCTHREADS();
   const int warp = tid >> 5, lane = tid & 31;
   if (warp < 10) fx_row_store(sh.S.mix[warp].w + (size_t)sh.w_set[warp] * fx::N_IN1, sh.w1[warp], lane);
   if (tid == 0) { sh.S.text = r.gx; sh.S.T = r.gT; }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   fx_copy_words(g, &sh.S, sizeof(fx::State), tid);
   fx_copy_words(r.gx, &sh.X, sizeof(fx::TextState), tid);
 }
@@ -191,7 +192,7 @@ __device__ void fx_bit(FxShared& sh, int y, int lstmpr, int lstmex, int tid) {
   if (tid == 0) { bit_head(S, y, lstmpr, lstmex); bit_prepare_head(S); }
   if (tid >= 32 && tid < 32 + N_MAPS) { sh.clash[tid - 32] = 0; sh.res[tid - 32] = 0; }
   for (int k = tid; k < FX_SEEN; k += FX_THREADS) sh.seen[k] = 0ull;
-  __syncthreads();
+  JIT_SYNCTHREADS();
   FX_T(0);
   // ---- B: SGD on the cached rows (Mixer1::update), the two 16-wide final rows, the units' slices of the vectors
   for (int idx = tid; idx < 10 * (N_IN1 / 8); idx += FX_THREADS) {
@@ -226,7 +227,7 @@ __device__ void fx_bit(FxShared& sh, int y, int lstmpr, int lstmex, int tid) {
     S.in_off[lane] = ia0 - a0; S.ex_off[lane] = ie0 - e0;
     if (lane + 32 <= N_UNITS) { S.in_off[lane + 32] = ta + ia1 - a1; S.ex_off[lane + 32] = te + ie1 - e1; }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   FX_T(1);
   // ---- C: buckets every map context touches; the units that are one lane each
   if (tid < FX_MAP_LANES) {
@@ -243,7 +244,7 @@ __device__ void fx_bit(FxShared& sh, int y, int lstmpr, int lstmex, int tid) {
     else if (tid == FX_TID_W9 + 8) u = U_RCM;
     if (u >= 0) bit_unit(S, u);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   FX_T(2);
   // ---- D: the map contexts
   if (tid < FX_MAP_LANES) {
@@ -258,7 +259,7 @@ __device__ void fx_bit(FxShared& sh, int y, int lstmpr, int lstmex, int tid) {
       sh.res[id] = r;
     }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   FX_T(3);
   // ---- E: map epilogues, weight-set selection
   if (warp == 0) {
@@ -266,7 +267,7 @@ __device__ void fx_bit(FxShared& sh, int y, int lstmpr, int lstmex, int tid) {
     __syncwarp();
     if (lane == 0) bit_select(S);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   FX_T(4);
   // ---- F: the ten 512-wide dot products over the cached rows (a selector that moved: write back, load)
   {
@@ -292,17 +293,17 @@ __device__ void fx_bit(FxShared& sh, int y, int lstmpr, int lstmex, int tid) {
     acc = __reduce_add_sync(0xffffffffu, acc);
     if (lane == 0) sh.dots[warp] = acc;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   FX_T(5);
   // ---- G: squash, final mixers, APMs, exports
   if (warp == 0) fx_tail_warp(sh, lane);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   FX_T(6);
 }
 
 // Bulk: CTA b serves stream b of the launch group. Writes ext[t][0..430] for every bit t of the sub-chunk (the codes
 // the model holds BEFORE perceiving bit t) and, when a.ext_replay is given, copies the non-resident PAQ8 slots next to them.
-__global__ void __launch_bounds__(FX_THREADS, 1) fxcm_kernel(const ChunkArgs* __restrict__ args_all) {
+__global__ void __launch_bounds__(FX_THREADS, 1) fxcm_kernel(const ChunkArgs* __restrict__ args_all) { jit_entry(JK_FXCM);
   extern __shared__ __align__(16) unsigned char fx_raw[];
   FxShared& sh = *reinterpret_cast<FxShared*>(fx_raw);
   const ChunkArgs a = args_all[blockIdx.x];
@@ -328,7 +329,7 @@ __global__ void __launch_bounds__(FX_THREADS, 1) fxcm_kernel(const ChunkArgs* __
 // Lock-step: one bit per launch (the decoder's order), queued behind the mixer / LSTM update of the same bit. Lane 0 first
 // takes the LSTM's read-out of the NEXT bit (ByteMixer::Predict + Discretize, predictor.cpp:462-465); the codes for the next
 // Predict() land in ext_bit[0..430].
-__global__ void __launch_bounds__(FX_THREADS, 1) fxcm_bit_kernel(StreamState* st, fx::State* g, int y, int pretrain, u16* ext_bit, const u32* dbit) {
+__global__ void __launch_bounds__(FX_THREADS, 1) fxcm_bit_kernel(StreamState* st, fx::State* g, int y, int pretrain, u16* ext_bit, const u32* dbit) { jit_entry(JK_FXCM_BIT);
   if (dbit) y = (int)dbit[0];
   extern __shared__ __align__(16) unsigned char fx_raw[];
   FxShared& sh = *reinterpret_cast<FxShared*>(fx_raw);
@@ -336,7 +337,7 @@ __global__ void __launch_bounds__(FX_THREADS, 1) fxcm_bit_kernel(StreamState* st
   const FxGlobals gl = fx_load(sh, g, tid);
   float* probs = reinterpret_cast<float*>(sh.seen);     // free until fx_bit clears it: the 256 probabilities arrive side by side
   if (!pretrain && tid < 256) probs[tid] = st->lstm.bm.probs[tid];
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) {
     if (pretrain) { sh.dots[10] = sh.S.lstmpr; sh.dots[11] = sh.S.lstmex; }
     else {
@@ -347,9 +348,9 @@ __global__ void __launch_bounds__(FX_THREADS, 1) fxcm_bit_kernel(StreamState* st
       sh.dots[11] = ex;
     }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   const int lstmpr = sh.dots[10], lstmex = sh.dots[11];
-  __syncthreads();
+  JIT_SYNCTHREADS();
   fx_bit(sh, y, lstmpr, lstmex, tid);
   if (ext_bit) for (int k = tid; k < fx::N_OUT; k += FX_THREADS) ext_bit[k] = sh.S.codes[k];
   fx_store(sh, g, gl, tid);

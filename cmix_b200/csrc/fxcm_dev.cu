@@ -16,6 +16,10 @@ void fxcm_launch_bit(StreamState* st, fx::State* g, int y, int pretrain, u16* ex
   fxcm_bit_kernel<<<1, FX_THREADS, sizeof(FxShared), s>>>(st, g, y, pretrain, ext_bit, dbit);
 }
 
+#ifdef CMIXB200_JITTER
+JIT_MODULE(fxcm)
+#endif
+
 }  // namespace cmixb200
 
 #ifdef FX_PROF

@@ -29,6 +29,7 @@
 #include <cooperative_groups.h>
 
 #include "exact_math.h"
+#include "jitter.cuh"
 #include "small_models.cuh"
 #include "state.h"
 
@@ -167,7 +168,7 @@ __device__ void lstm_layer_forward(cgl::cluster_group& cluster, LstmState& S, in
     if (tid < LCPC) lcp_async4(dst + in_sizep * LCPC + tid, ssrc + tid);
   }
   lcp_async_wait();
-  __syncthreads();
+  JIT_SYNCTHREADS();
   L_PROF(4);
   // ---- 75 serial chains out of shared memory ----
   float f = 0.0f;
@@ -182,12 +183,12 @@ __device__ void lstm_layer_forward(cgl::cluster_group& cluster, LstmState& S, in
     }
   }
   L_PROF(5);
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
   L_PROF(7);
   // ---- RMS norm: every CTA computes the three sums redundantly (back to front, _Expr::sum()):
   //      squares in parallel, then one FADD chain per gate ----
   for (int k = tid; k < 3 * LC; k += LSTM_THREADS) { const float v = sh.gat[k / LC][k % LC]; sh.prod[k / LC][k % LC] = XM_FMUL(v, v); }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid < 96 && (tid & 31) == 0) {
     const int g = tid >> 5;
     const float ss = sum_back_to_front(sh.prod[g], LC);
@@ -195,7 +196,7 @@ __device__ void lstm_layer_forward(cgl::cluster_group& cluster, LstmState& S, in
     sh.scal[g] = iv;
     if (rank == 0) P.ivar[l][g][e] = iv;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   L_PROF(9);
   if (tid < 96 && (tid & 31) < LCPC) {
     const int g = tid >> 5, i = tid & 31, cell = LCPC * rank + i;
@@ -206,7 +207,7 @@ __device__ void lstm_layer_forward(cgl::cluster_group& cluster, LstmState& S, in
     P.state[l][g][(size_t)e * LC + cell] = s;
     sh.act[g][i] = s;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   L_PROF(10);
   if (tid < LCPC) {
     const int i = tid, cell = LCPC * rank + i;
@@ -227,10 +228,10 @@ __device__ void lstm_layer_forward(cgl::cluster_group& cluster, LstmState& S, in
       rh[l * LC + cell] = h;
     }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) P.lepoch[l] = (e + 1 == LH) ? 0 : e + 1;
   L_PROF(8);
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
   L_PROF(7);
 }
 
@@ -247,7 +248,7 @@ __device__ void lstm_predict(cgl::cluster_group& cluster, LstmState& S, unsigned
       if (l == 1 && tid >= 256 && tid < 256 + LC) in[V + LC + (tid - 256)] = sh.hid[tid - 256];
     }
     __threadfence();
-    cluster.sync();
+    jit_cluster_sync(cluster, JIT_HERE);
     L_PROF(7);
     lstm_layer_forward(cluster, S, l, (int)input, sh, rank, tid, prof, tprev);
   }
@@ -258,41 +259,41 @@ __device__ void lstm_predict(cgl::cluster_group& cluster, LstmState& S, unsigned
   const int nrow = max(0, r1 - r0);
   for (int k = tid; k < nrow * HW; k += LSTM_THREADS) lcp_async4(sh.pool + k, W + (size_t)r0 * HW + k);
   lcp_async_wait();
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid < nrow) {
     const float* wr = sh.pool + (size_t)tid * HW;
     const float sum = chain_strided(0.0f, sh.hid, wr, HW, 1);
 #pragma unroll 1
     for (int c = 0; c < LSTM_CTAS; ++c) { float* rl = cluster.map_shared_rank(sh.logits, c); rl[r0 + tid] = sum; }
   }
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
   // every CTA: max(0, max_i), exp, front-to-back total, divide (identical results everywhere)
   float mx = 0.0f;
   for (int i = tid; i < V; i += LSTM_THREADS) mx = fmaxf(mx, sh.logits[i]);
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   if ((tid & 31) == 0) sh.err[tid >> 5] = mx;
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) { float m2 = 0.0f; for (int w = 0; w < LSTM_THREADS / 32; ++w) m2 = fmaxf(m2, sh.err[w]); sh.scal[4] = m2; }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   const float max_out = sh.scal[4];
   for (int i = tid; i < V; i += LSTM_THREADS) sh.logits[i] = lt_expf(XM_FSUB(sh.logits[i], max_out));
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) {
     float total = sh.logits[0];
 #pragma unroll 8
     for (int i = 1; i < V; ++i) total = XM_FADD(total, sh.logits[i]);
     sh.scal[5] = total;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   for (int i = tid; i < V; i += LSTM_THREADS) {
     const float o = XM_FDIV(sh.logits[i], sh.scal[5]);
     sh.logits[i] = o;
     if (rank == 0) P.output[(size_t)e * V + i] = o;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) P.epoch = (e + 1 == LH) ? 0 : e + 1;
   __threadfence();
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
   L_PROF(6);
 }
 
@@ -321,7 +322,7 @@ __device__ void lstm_layer_backward(cgl::cluster_group& cluster, LstmState& S, i
     if (ep > 0) { se = XM_FMUL(se, fs); stored = 0.0f; }
   }
   if (tid == 0 && ep == 0) { if (P.update_steps[l] < 3000) ++P.update_steps[l]; }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   // per gate: beta_u/gamma_u accumulation, scale by gamma*ivar, all-gather for the RMS-norm backward sum
   float escaled = 0.0f;
   if (tid < 96 && (tid & 31) < LCPC) {
@@ -342,14 +343,14 @@ __device__ void lstm_layer_backward(cgl::cluster_group& cluster, LstmState& S, i
   // the full norm vector of this step straight from HBM/L2 into registers while the all-gather lands
   float nv[2] = {0.0f, 0.0f};
   for (int k = tid, q = 0; k < 3 * LC; k += LSTM_THREADS, ++q) nv[q] = P.norm[l][k / LC][(size_t)ep * LC + (k % LC)];
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
   for (int k = tid, q = 0; k < 3 * LC; k += LSTM_THREADS, ++q) sh.prod[k / LC][k % LC] = XM_FMUL(sh.gat[k / LC][k % LC], nv[q]);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid < 96 && (tid & 31) == 0) {
     const int g = tid >> 5;
     sh.scal[g] = XM_FDIV(sum_back_to_front(sh.prod[g], LC), (float)LC);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   // no second cluster barrier: the sums read gat/prod only, and gat2 (written next, remotely) is not read again
   // before the barrier below; gat itself is next overwritten after that barrier.
   if (tid < 96 && (tid & 31) < LCPC) {
@@ -362,7 +363,7 @@ __device__ void lstm_layer_backward(cgl::cluster_group& cluster, LstmState& S, i
       rd[g][cell] = e;
     }
   }
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
   // transposed mat-vecs for the own 25 columns: hidden_error (layer below) and stored_error (previous step)
   float f1 = 0.0f, f2 = 0.0f;
   if (tid < 192 && (tid & 31) < LCPC) {
@@ -377,7 +378,7 @@ __device__ void lstm_layer_backward(cgl::cluster_group& cluster, LstmState& S, i
       sh.pool[LSTM_POOL_FLOATS - 256 + wv * 32 + i] = 0.0f;
     }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid < LCPC) {
     const int i = tid;
     const float* sc = sh.pool + LSTM_POOL_FLOATS - 256;
@@ -387,7 +388,7 @@ __device__ void lstm_layer_backward(cgl::cluster_group& cluster, LstmState& S, i
     *stored_reg = clipf(stored, kClip);
     *he_reg = clipf(he, kClip);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
 }
 
 // Weight-gradient accumulation in the reference's time order + Adam (lstm-layer.cpp:11-32,182-196).
@@ -403,20 +404,20 @@ __device__ void lstm_apply_updates(LstmState& S, LstmShared& sh, int rank, int t
     const float* ad = P.adam + 4 * P.update_steps[l];
     const float alpha = ad[0], bc1 = ad[1], bc2 = ad[2];
     const int in_size = P.in_size[l], row = in_size + V;
-    __syncthreads();
+    JIT_SYNCTHREADS();
     for (int k = tid; k < 3 * LH * LCPC; k += LSTM_THREADS) {
       const int g = k / (LH * LCPC), r = k - g * LH * LCPC, ep = r / LCPC, i = r - ep * LCPC;
       err_s[k] = P.err[l][g][(size_t)ep * LC + LCPC * rank + i];
     }
     for (int c0 = 0; c0 < row; c0 += TILE) {
       const int nc = min(TILE, row - c0);
-      __syncthreads();
+      JIT_SYNCTHREADS();
       // dense columns of this tile: inputs of all 100 steps
       for (int k = tid; k < LH * TILE; k += LSTM_THREADS) {
         const int ep = k / TILE, c = k - ep * TILE, col = c0 + c;
         in_t[k] = (c < nc && col >= V) ? P.input[l][(size_t)ep * in_size + (col - V)] : 0.0f;
       }
-      __syncthreads();
+      JIT_SYNCTHREADS();
       for (int k = tid; k < 3 * nc * LCPC; k += LSTM_THREADS) {
         const int g = k / (nc * LCPC), r = k - g * nc * LCPC, c = r / LCPC, i = r - c * LCPC, col = c0 + c;
         const float* es = err_s + (size_t)g * LH * LCPC + i;
@@ -456,7 +457,7 @@ __device__ void lstm_apply_updates(LstmState& S, LstmShared& sh, int rank, int t
       }
     }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
 }
 
 // ByteMixer::ByteUpdate -> Lstm::SetInput + Lstm::Perceive + Lstm::Predict (byte-mixer.cpp:22-38,
@@ -486,16 +487,16 @@ __device__ void lstm_load_cache(LstmState& S, LstmShared& sh, int rank, int tid)
   if (tid < LSTM_HORIZON) sh.hist[tid] = S.input_history[tid];
   for (int i = tid; i < 256; i += LSTM_THREADS) { sh.bmap[i] = S.byte_map[i]; sh.vocab[i] = S.vocab[i]; sh.probs256[i] = S.bm.probs[i]; }
   for (int j = tid; j < LSTM_HID; j += LSTM_THREADS) sh.hid[j] = S.hidden[j];
-  __syncthreads();
+  JIT_SYNCTHREADS();
   {   // softmax output of the previous byte (needed by the output-layer SGD)
     const int V = sh.P.V, le = sh.P.epoch == 0 ? LSTM_HORIZON - 1 : sh.P.epoch - 1;
     for (int i = tid; i < V; i += LSTM_THREADS) sh.logits[i] = sh.P.output[(size_t)le * V + i];
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
 }
 // ... and write the mutable part back (kernel epilogue).
 __device__ void lstm_store_cache(LstmState& S, LstmShared& sh, int rank, int tid) {
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid < LCPC) { S.layer[0].state[LCPC * rank + tid] = sh.cst[0][tid]; S.layer[1].state[LCPC * rank + tid] = sh.cst[1][tid]; }
   if (rank == 0) {
     if (tid == 0) {
@@ -528,14 +529,14 @@ __device__ void lstm_byte_update(cgl::cluster_group& cluster, LstmState& S, cons
     P.input[0][(size_t)epoch * P.in_size[0] + k] = a;
     P.input[1][(size_t)epoch * P.in_size[1] + k] = a;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) sh.hist[last_epoch] = input;
-  __syncthreads();
+  JIT_SYNCTHREADS();
   L_PROF(0);
   if (epoch == 0) {
     // ------------------------------ truncated BPTT ------------------------------
     __threadfence();
-    cluster.sync();                                     // rank 0's SetInput writes are visible to every CTA
+    jit_cluster_sync(cluster, JIT_HERE);                                     // rank 0's SetInput writes are visible to every CTA
     if (tid < LH) sh.sym[tid] = tid == 0 ? old_input : (int)sh.hist[tid - 1];
     float gamma_u[2] = {0.0f, 0.0f}, beta_u[2] = {0.0f, 0.0f};
     float he_reg = 0.0f, stored_reg[2] = {0.0f, 0.0f}, se_reg[2] = {0.0f, 0.0f};
@@ -554,20 +555,20 @@ __device__ void lstm_byte_update(cgl::cluster_group& cluster, LstmState& S, cons
       }
     }
     lcp_async_wait();
-    __syncthreads();
+    JIT_SYNCTHREADS();
     for (int ep = LH - 1; ep >= 0; --ep) {
       const float* out = P.output + (size_t)ep * V;
       const float* W = P.out_w + (size_t)ep * V * HW;
       for (int i = tid; i < V; i += LSTM_THREADS) sh.err[i] = ((unsigned)i == sh.hist[ep]) ? XM_FSUB(out[i], 1.0f) : out[i];
       for (int l = 1; l >= 0; --l) {
         // slice of W_o[ep]: columns l*200 + own 25 cells, all V rows
-        __syncthreads();
+        JIT_SYNCTHREADS();
         for (int k = tid; k < V * LCPC; k += LSTM_THREADS) {
           const int i = k / LCPC, jj = k - i * LCPC;
           lcp_async4(wo_s + k, W + (size_t)i * HW + l * LC + LCPC * rank + jj);
         }
         lcp_async_wait();
-        __syncthreads();
+        JIT_SYNCTHREADS();
         if (tid < LCPC) {
           float he = he_reg;
           const float* wc = wo_s + tid;
@@ -586,7 +587,7 @@ __device__ void lstm_byte_update(cgl::cluster_group& cluster, LstmState& S, cons
     L_PROF(1);
     lstm_apply_updates(S, sh, rank, tid, gamma_u, beta_u);
     __threadfence();
-    cluster.sync();
+    jit_cluster_sync(cluster, JIT_HERE);
     L_PROF(2);
   }
   // ---- output layer SGD (lstm.cpp:112-116): W_o[epoch] = W_o[last_epoch] - (lr*err_i) * hidden, own rows ----
@@ -597,18 +598,18 @@ __device__ void lstm_byte_update(cgl::cluster_group& cluster, LstmState& S, cons
     float* We = P.out_w + (size_t)epoch * V * HW;
     // sh.logits still holds the softmax output of the previous byte (output_[last_epoch])
     for (int i = tid; i < V; i += LSTM_THREADS) sh.err[i] = XM_FMUL(0.03f, ((unsigned)i == input) ? XM_FSUB(sh.logits[i], 1.0f) : sh.logits[i]);
-    __syncthreads();
+    JIT_SYNCTHREADS();
     for (int idx = r0 * HW + tid; idx < r1 * HW; idx += LSTM_THREADS) {
       const int i = idx / HW, j = idx - i * HW;
       We[idx] = XM_FSUB(Wl[idx], XM_FMUL(sh.err[i], sh.hid[j]));
     }
-    __syncthreads();
+    JIT_SYNCTHREADS();
   }
   L_PROF(3);
   lstm_predict(cluster, S, input, sh, rank, tid, prof, tprev);
   // ByteMixer: scatter back to 256 bytes; ByteModel::ByteUpdate resets the range
   if (tid < 256) sh.probs256[tid] = sh.vocab[tid] ? sh.logits[sh.bmap[tid]] : 0.0f;
-  __syncthreads();
+  JIT_SYNCTHREADS();
 }
 
 // Bit-level read-out of the byte distribution (ByteModel::Predict + the override test of
@@ -632,7 +633,7 @@ __device__ void bm_perceive(ByteModelState& b, int bit) {
 }
 
 __global__ void __cluster_dims__(LSTM_CTAS, 1, 1) __launch_bounds__(LSTM_THREADS, 1)
-lstm_kernel(const ChunkArgs* __restrict__ args_all, Tables T) {
+lstm_kernel(const ChunkArgs* __restrict__ args_all, Tables T) { jit_entry(JK_LSTM);
   cgl::cluster_group cluster = cgl::this_cluster();
   const int rank = (int)cluster.block_rank();
   const ChunkArgs a = args_all[blockIdx.x / LSTM_CTAS];
@@ -674,18 +675,18 @@ lstm_kernel(const ChunkArgs* __restrict__ args_all, Tables T) {
   }
   lstm_store_cache(S, sh, rank, tid);
   __threadfence();
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
 }
 
 // Lock-step halves.
 // Lock-step Predict(), producer half: CTA 0 = the 54 small models + contexts (small_models.cuh), CTA 1 = the
 // LSTM's bit read-out (ByteModel::Predict, byte-model.cpp:8-15). Independent of each other, one launch.
-__global__ void __launch_bounds__(64, 1) lock_predict_inputs_kernel(StreamState* st, Tables T) {
+__global__ void __launch_bounds__(64, 1) lock_predict_inputs_kernel(StreamState* st, Tables T) { jit_entry(JK_LSTM_INPUTS);
   if (blockIdx.x == 1) {            // the LSTM's bit read-out: the 256 probabilities come in side by side, the sums stay one serial chain
     __shared__ float probs[256];
     ByteModelState& b = st->lstm.bm;
     for (int i = threadIdx.x; i < 256; i += 64) probs[i] = b.probs[i];
-    __syncthreads();
+    JIT_SYNCTHREADS();
     if (threadIdx.x == 0) {
       const float p = bytemodel_predict(probs, b.bot, b.top, &b.ex);
       st->lstm_override = (p == 0.0f || p == 1.0f) ? p : -1.0f;
@@ -698,11 +699,11 @@ __global__ void __launch_bounds__(64, 1) lock_predict_inputs_kernel(StreamState*
   const int tid = threadIdx.x;
   for (int i = tid; i < 256; i += 64) { sh.bracket_probs[i] = s.bracket_bm.probs[i]; sh.ppmd_probs[i] = s.ppmd_bm.probs[i]; }
   if (tid == 0) small_refresh_tables(s, sh);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   small_predict(st->small, T, sh, st->small_x, st->sel, tid);
 }
 __global__ void __cluster_dims__(LSTM_CTAS, 1, 1) __launch_bounds__(LSTM_THREADS, 1)
-lstm_byte_kernel(StreamState* st, u32 byte, const float* ppmd, const u32* dbit = nullptr) {
+lstm_byte_kernel(StreamState* st, u32 byte, const float* ppmd, const u32* dbit = nullptr) { jit_entry(JK_LSTM_BYTE);
   if (dbit) byte = dbit[1];
   cgl::cluster_group cluster = cgl::this_cluster();
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -713,7 +714,7 @@ lstm_byte_kernel(StreamState* st, u32 byte, const float* ppmd, const u32* dbit =
   lstm_byte_update(cluster, st->lstm, ppmd, byte, sh, rank, threadIdx.x, nullptr, &tprev);
   lstm_store_cache(st->lstm, sh, rank, threadIdx.x);
   __threadfence();
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
 }
 
 #undef LC

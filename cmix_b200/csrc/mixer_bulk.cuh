@@ -36,6 +36,7 @@
 //   through distributed shared memory), so CTA 1's extra-input prefix overlaps CTA 0's loop and no
 //   cluster barrier or cluster fence is ever executed inside the bit loop.
 #pragma once
+#include "jitter.cuh"
 #include "mixer.cuh"
 
 namespace cmixb200 {
@@ -46,10 +47,11 @@ enum { MIX_NBUF = 20, MIX_RING = 4, MIX_M_WARPS = 11, MIX_M_THREADS = MIX_M_WARP
        ROW_PITCH_S = 2108,     // shared-memory row pitch: 527 float4 (odd) -> LDS.128 conflict-free across lanes
        K_SAME = 0, K_SWAP = 1, K_LATE_SWITCH = 3, T_ELEMS = 819 };
 
-__device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void spin_until_ge(volatile u32* p, u32 v) {
+__device__ __forceinline__ void named_sync(int id, int count, int site) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); jit_point(site); }
+__device__ __forceinline__ void named_arrive(int id, int count, int site) { jit_point(site); asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+__device__ __forceinline__ void spin_until_ge(volatile u32* p, u32 v, int site) {
   while (*p < v) { }
+  jit_point(site);
 }
 
 // "LL" message slots (as in NCCL's low-latency protocol): a float and its sequence number are written
@@ -58,9 +60,10 @@ __device__ __forceinline__ void spin_until_ge(volatile u32* p, u32 v) {
 __device__ __forceinline__ void ll_store(uint2* slot, float v, u32 seq) {
   *reinterpret_cast<volatile unsigned long long*>(slot) = ((unsigned long long)seq << 32) | (unsigned long long)__float_as_uint(v);
 }
-__device__ __forceinline__ float ll_wait(const uint2* slot, u32 seq) {
+__device__ __forceinline__ float ll_wait(const uint2* slot, u32 seq, int site) {
   unsigned long long m;
   do { m = *reinterpret_cast<const volatile unsigned long long*>(slot); } while ((u32)(m >> 32) != seq);
+  jit_point(site);
   return __uint_as_float((u32)m);
 }
 
@@ -72,11 +75,12 @@ __device__ __forceinline__ void mbar_init(unsigned long long* bar, int count) {
 __device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
+__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity, int site) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "W: mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
       "@!p bra W;\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+  jit_point(site);
 }
 __device__ __forceinline__ void tma_load_row(void* smem_dst, const void* gmem_src, unsigned bytes, unsigned long long* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -169,7 +173,7 @@ __device__ __forceinline__ void movers_update(MixBulkShared& sh, int m0, int mti
 #pragma unroll 1
   for (int c = 0; c < MIX_CHUNKS; ++c) {
     movers_update_chunk(sh, m0, mtid >> 5, mtid & 31, par_prev, xprev, c);
-    named_sync(BAR_MOVERS, MIX_M_THREADS);
+    named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
     if (mtid == 0) sh.chunk_seq[c] = seq;
   }
 }
@@ -217,9 +221,9 @@ __device__ __forceinline__ void run_row_jobs(MixBulkShared& sh, StreamState* st,
     bool any_load = false;
 #pragma unroll 1
     for (int j = 0; j < nj; ++j) any_load |= sh.jobs[j].do_load != 0;
-    if (any_load) { mbar_wait(&sh.row_bar, sh.row_bar_phase & 1); sh.row_bar_phase++; }
+    if (any_load) { mbar_wait(&sh.row_bar, sh.row_bar_phase & 1, JIT_HERE); sh.row_bar_phase++; }
   }
-  named_sync(BAR_MOVERS, MIX_M_THREADS);
+  named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
 }
 
 // movers: the learning-rate factor of bit t for local mixer i, on the step counters kept in shared memory
@@ -232,7 +236,7 @@ __device__ __forceinline__ void plan_rate(MixBulkShared& sh, int par, int i, flo
 }
 
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(MIX_THREADS, 1)
-mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
+mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) { jit_entry(JK_MIX);
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
   const ChunkArgs a = args_all[blockIdx.x / 2];
@@ -264,8 +268,8 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
     for (int i = 0; i <= N_L1; ++i) { const int n = i < N_L1 ? L1_IN + i : L2_IN; for (int c = 0; c < n; ++c) sh.emap[e++] = (unsigned short)((i << 8) | c); }
   }
   for (int k = tid; k < 4097; k += MIX_THREADS) sh.lut12[k] = T.lut12[k];
-  __syncthreads();
-  cluster.sync();
+  JIT_SYNCTHREADS();
+  jit_cluster_sync(cluster, JIT_HERE);
 
   if (warp == MIX_C_WARP) {
     // =============================== C warp ===============================
@@ -276,7 +280,7 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
     for (u64 t = 0; t < n_bits; ++t) {
       const int par = (int)(t & 1), r = (int)(t & (MIX_RING - 1));
       const int bit = (a.bytes[t >> 3] >> (7 - (t & 7))) & 1;
-      named_sync(BAR_READY0 + par, MIX_CM);
+      named_sync(BAR_READY0 + par, MIX_CM, JIT_HERE);
       MIX_PROF(pc_on, pb + 0);
       const float* x = sh.x[t % 3];
       float* row = sh.rows[lane < MIX_PER_CTA ? sh.plan_buf[par][lane] : 0];
@@ -288,6 +292,7 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
 #pragma unroll 1
         for (int c = 0; c < MIX_CHUNKS; ++c) {
           while (sh.chunk_seq[c] < (u32)t) { }            // the movers have applied bit t-1's step to this chunk
+          jit_point(JIT_HERE);
           if (lane < MIX_PER_CTA) main = chain_chunk(x4, w4, c * MIX_CHUNK4, chain_chunk_end(c), main);
         }
         if (lane < MIX_PER_CTA) main = chain_tail(x, row, main);
@@ -302,17 +307,17 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
       if (rank == 1) {
 #pragma unroll 1
         for (int k = 0; k < MIX_PER_CTA; ++k) {
-          const float ck = ll_wait(&sh.ring_in[r][k], (u32)(t + 1));
+          const float ck = ll_wait(&sh.ring_in[r][k], (u32)(t + 1), JIT_HERE);
           if (lane == k) sh.cext[par][k] = ck;
           if (lane < MIX_PER_CTA) e = XM_FADD(e, XM_FMUL(ck, row[N_INPUTS + k]));
         }
         if (lane == 0) sh0->peer_progress = (u32)(t + 1);
         kbase = MIX_PER_CTA;
       } else {
-        if (lane == 0 && t >= MIX_RING) { spin_until_ge(&sh.peer_progress, (u32)(t + 1 - MIX_RING)); spin_until_ge(&sh.t_consumed, (u32)(t + 1 - MIX_RING)); }
+        if (lane == 0 && t >= MIX_RING) { spin_until_ge(&sh.peer_progress, (u32)(t + 1 - MIX_RING), JIT_HERE); spin_until_ge(&sh.t_consumed, (u32)(t + 1 - MIX_RING), JIT_HERE); }
         __syncwarp();
       }
-      if (rank == 1 && lane == 0 && t >= MIX_RING) spin_until_ge(&sh.t_consumed, (u32)(t + 1 - MIX_RING));
+      if (rank == 1 && lane == 0 && t >= MIX_RING) spin_until_ge(&sh.t_consumed, (u32)(t + 1 - MIX_RING), JIT_HERE);
       __syncwarp();
       MIX_PROF(pc_on, pb + 2);
       float wnext = lane < MIX_PER_CTA ? row[N_INPUTS + kbase] : 0.0f;
@@ -342,7 +347,7 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
       }
       __syncwarp();
       MIX_PROF(pc_on, pb + 4);
-      named_arrive(BAR_COEFF0 + par, MIX_CM);
+      named_arrive(BAR_COEFF0 + par, MIX_CM, JIT_HERE);
       MIX_PROF(pc_on, pb + 5);
     }
     MIX_PROF_DUMP(pc_on, pb, 6);
@@ -362,7 +367,7 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
         if (mtid >= 64 && mtid < 64 + MIX_PER_CTA && !(rank == 0 && mtid - 64 == 12))
           sh.want[mtid - 64] = resolve_slot(st->mixer[m0 + mtid - 64], a.sel[t * SEL_PITCH + m0 + mtid - 64]);
         stage_inputs<MIX_M_THREADS>(sh.x[t % 3], sh.lut12, a.ext ? a.ext + t * N_EXT : nullptr, a.small_x + t * SMALL_X_PITCH, a.lstm_x[2 * t], mtid);
-        named_sync(BAR_MOVERS, MIX_M_THREADS);
+        named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
         MIX_PROF(pm_on, 20);
         if (mtid == 0) {
           if (rank == 0) { const u32 ax = aux_context(sh.x[t % 3]); sh.sel[par][12] = ax; sh.want[12] = resolve_slot(st->mixer[12], ax); }
@@ -394,22 +399,22 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
           }
           sh.n_jobs = nj; sh.n_late = nlate;
         }
-        named_sync(BAR_MOVERS, MIX_M_THREADS);
+        named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
         MIX_PROF(pm_on, 21);
         run_row_jobs(sh, st, m0, mtid);
         const float decay = a.decay[t];
         if (mtid < MIX_PER_CTA && sh.kind[mtid] != K_LATE_SWITCH) plan_rate(sh, par, mtid, decay, my_lr);
-        named_sync(BAR_MOVERS, MIX_M_THREADS);
+        named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
         MIX_PROF(pm_on, 22);
         if (sh.n_late) {
           // rows that must carry bit t-1's step BEFORE bit t's chain: shrink due, or single-buffered switch
-          if (t > 0) { named_sync(BAR_COEFF0 + parp, MIX_CM); coeff_synced = true; }
+          if (t > 0) { named_sync(BAR_COEFF0 + parp, MIX_CM, JIT_HERE); coeff_synced = true; }
           if (mtid < MIX_PER_CTA) {
             if (t > 0 && sh.kind[mtid] == K_LATE_SWITCH && sh.tag[sh.buf_cur[mtid]] != 0xffffffffu) sh.mupd[mtid] = sh.buf_cur[mtid];
           }
-          named_sync(BAR_MOVERS, MIX_M_THREADS);
+          named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
           if (t > 0) movers_update(sh, m0, mtid, parp, sh.x[(t + 2) % 3], (u32)t);
-          named_sync(BAR_MOVERS, MIX_M_THREADS);
+          named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
           if (mtid == 0) {
             int nj = 0;
 #pragma unroll 1
@@ -424,19 +429,19 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
             }
             sh.n_jobs = nj;
           }
-          named_sync(BAR_MOVERS, MIX_M_THREADS);
+          named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
           run_row_jobs(sh, st, m0, mtid);
           if (mtid < MIX_PER_CTA && sh.kind[mtid] == K_LATE_SWITCH) plan_rate(sh, par, mtid, decay, my_lr);
-          named_sync(BAR_MOVERS, MIX_M_THREADS);
+          named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
         }
         MIX_PROF(pm_on, 23);
-        named_arrive(BAR_READY0 + par, MIX_CM);
+        named_arrive(BAR_READY0 + par, MIX_CM, JIT_HERE);
       }
       // ---- bit t-1's step for the rows that were switched away (or, at the end, for all rows) ----
       if (t > 0) {
-        if (!coeff_synced) named_sync(BAR_COEFF0 + parp, MIX_CM);
+        if (!coeff_synced) named_sync(BAR_COEFF0 + parp, MIX_CM, JIT_HERE);
         MIX_PROF(pm_on, 24);
-        if (t == n_bits) { if (mtid < MIX_PER_CTA) sh.mupd[mtid] = sh.buf_cur[mtid]; named_sync(BAR_MOVERS, MIX_M_THREADS); }
+        if (t == n_bits) { if (mtid < MIX_PER_CTA) sh.mupd[mtid] = sh.buf_cur[mtid]; named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE); }
         movers_update(sh, m0, mtid, parp, sh.x[(t + 2) % 3], (u32)t);
         MIX_PROF(pm_on, 25);
       }
@@ -458,7 +463,7 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
       }
       sh.n_jobs = nj;
     }
-    named_sync(BAR_MOVERS, MIX_M_THREADS);
+    named_sync(BAR_MOVERS, MIX_M_THREADS, JIT_HERE);
     run_row_jobs(sh, st, m0, mtid);
     if (mtid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   } else if (rank == 0 && warp == MIX_T_WARP) {
@@ -527,7 +532,7 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
       MIX_PROF(pt_on, 26);
       {
         float c = 0.0f;
-        if (lane < N_L0 + N_AUX) c = ll_wait(&sh.ring_t[r][lane], (u32)(t + 1));
+        if (lane < N_L0 + N_AUX) c = ll_wait(&sh.ring_t[r][lane], (u32)(t + 1), JIT_HERE);
         if (lane < N_L0) { sh.in1[lane] = c; sh.in2[lane] = c; }
         else if (lane < N_L0 + N_AUX) { sh.in1[lane] = c; sh.in2[N_L1 + lane] = c; }
       }
@@ -598,8 +603,8 @@ mix_kernel_v3(const ChunkArgs* __restrict__ args_all, Tables T) {
     }
     if (lane == 0) { sse.j = sj; sse.pc = spc; sse.ffl = sffl; st->bits_done += n_bits; }
   }
-  __syncthreads();
-  cluster.sync();
+  JIT_SYNCTHREADS();
+  jit_cluster_sync(cluster, JIT_HERE);
 }
 
 }  // namespace cmixb200

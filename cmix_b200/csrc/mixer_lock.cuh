@@ -19,25 +19,25 @@ struct LockRowShared {
 };
 
 __global__ void __launch_bounds__(256, 1)
-mix_predict_rows_kernel(StreamState* st, Tables T, const u16* ext /* device, N_EXT codes or null */) {
+mix_predict_rows_kernel(StreamState* st, Tables T, const u16* ext /* device, N_EXT codes or null */) { jit_entry(JK_MIX_ROWS);
   __shared__ LockRowShared sh;
   const int tid = threadIdx.x, i = blockIdx.x;
   stage_inputs<256>(sh.x, T.lut12, ext, st->small_x, st->lstm_x, tid);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) {
     const u32 sel = i == 12 ? aux_context(sh.x) : st->sel[i];
     const u32 s = resolve_slot(st->mixer[i], sel);
     st->slot[i] = s;
     sh.slot = s;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   {
     const float4* g = reinterpret_cast<const float4*>(st->mixer[i].rows + (size_t)sh.slot * ROW_PITCH_L0);
     float4* d = reinterpret_cast<float4*>(sh.row);
     for (int k = tid; k < ROW_PITCH_L0 / 4; k += 256) d[k] = g[k];
   }
   if (i == 0) for (int k = tid; k < N_INPUTS; k += 256) st->x[k] = sh.x[k];
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) {
     const float4* x4 = reinterpret_cast<const float4*>(sh.x);
     const float4* w4 = reinterpret_cast<const float4*>(sh.row);
@@ -61,13 +61,13 @@ struct LockFinalShared {
 };
 
 __global__ void __launch_bounds__(MIX_THREADS, 1)
-mix_predict_final_kernel(StreamState* st, Tables T) {
+mix_predict_final_kernel(StreamState* st, Tables T) { jit_entry(JK_MIX_FINAL);
   __shared__ LockFinalShared sh;
   const int tid = threadIdx.x, lane = tid & 31;
   if (tid < N_L0) sh.mains[tid] = st->mains[tid];
   if (tid >= 32 && tid < 32 + N_AUX) sh.aux[tid - 32] = st->x[tid == 32 ? 433 : (tid == 33 ? 2024 : 2077)];
   if (tid >= N_L0 && tid < N_MIXERS) { const u32 s = resolve_slot(st->mixer[tid], st->sel[tid]); st->slot[tid] = s; sh.slot1[tid - N_L0] = s; }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   for (int k = tid; k < (N_L1 + 1) * ROW_PITCH_L1; k += MIX_THREADS) {
     const int i = k / ROW_PITCH_L1, c = k - i * ROW_PITCH_L1;
     sh.l1row[i][c] = st->mixer[N_L0 + i].rows[(size_t)sh.slot1[i] * ROW_PITCH_L1 + c];
@@ -76,7 +76,7 @@ mix_predict_final_kernel(StreamState* st, Tables T) {
     const int i = k / N_L0, c = k - i * N_L0;
     sh.we[i][c] = st->mixer[i].rows[(size_t)st->slot[i] * ROW_PITCH_L0 + N_INPUTS + c];
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid < 32) {
     // layer 0's clamped outputs are the first inputs of layers 1 and 2, followed by the 3 auxiliary inputs
     const float p0 = substitute<N_L0>(lane < N_L0 ? sh.mains[lane] : 0.0f, sh.we[lane], T, sh.in1, sh.in2, lane);
@@ -105,7 +105,7 @@ mix_predict_final_kernel(StreamState* st, Tables T) {
       st->last_p = st->lstm_override >= 0.0f ? st->lstm_override : p;
     }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid < N_L0) st->extras0[tid] = sh.in1[tid];
   if (tid < N_L1) st->extras1[tid] = sh.l1extra[tid];
   if (tid < L2_IN) st->in2[tid] = sh.in2[tid];
@@ -117,7 +117,7 @@ mix_predict_final_kernel(StreamState* st, Tables T) {
 // layers 1-2, the SSE update and the step counter; CTA 27 the LSTM read-out's bit update
 // (ByteModel::Perceive, byte-model.cpp:17-30).
 __global__ void __launch_bounds__(MIX_THREADS, 1)
-mix_perceive_kernel(StreamState* st, int bit, float decay_base, const u32* dbit = nullptr) {
+mix_perceive_kernel(StreamState* st, int bit, float decay_base, const u32* dbit = nullptr) { jit_entry(JK_MIX_PERCEIVE);
   if (dbit) {                            // decode loop: the bit and the step's decay factor come from the device
     const DecodeState* ds = reinterpret_cast<const DecodeState*>(dbit);
     bit = (int)ds->bit;
@@ -135,7 +135,7 @@ mix_perceive_kernel(StreamState* st, int bit, float decay_base, const u32* dbit 
       upd[0] = sgd_coeff(mixer_rate(decay_base, m.lr, rs, ms), st->mix_p[i], bit);
       mixer_step(rs, ms, steps, m.max_steps, shrink[0]);
     }
-    __syncthreads();
+    JIT_SYNCTHREADS();
     float* row = m.rows + (size_t)st->slot[i] * ROW_PITCH_L0;
     const int n = N_INPUTS + i;
     const float u = upd[0];
@@ -160,7 +160,7 @@ mix_perceive_kernel(StreamState* st, int bit, float decay_base, const u32* dbit 
     sse_learn(c, bit, S.s6 + (size_t)S.i6 * 8, S.s7 + (size_t)S.i7 * 8, &S.x1[S.ix1], &S.x2[S.ix2]);
     sse_advance(S.j, S.pc, S.ffl, bit);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   for (int k = tid; k < (N_L1 + 1) * ROW_PITCH_L1; k += MIX_THREADS) {
     const int i = k / ROW_PITCH_L1, c = k - i * ROW_PITCH_L1;
     const int mi = N_L0 + i;

@@ -35,6 +35,7 @@
 // PAQ8 is a producer like FXCM: it depends on the coded bytes only and writes 1591 codes per bit into the `ext` scratch.
 #pragma once
 #include <cooperative_groups.h>
+#include "jitter.cuh"
 #include "paq8_top.h"
 #include "state.h"
 
@@ -620,12 +621,12 @@ static_assert(p8::N_IN % 8 == 0 && p8::N_IN / 8 <= 7 * 32, "a weight row is at m
 
 // named barrier 2: the model warps signal "the state the 19 order-independent selector sets read is final" (arrive), the
 // first SGD warp waits for it (sync) and computes those sets beside the apply phase
-__device__ __forceinline__ void p8_signal_selects() { asm volatile("bar.arrive 2, 416;" ::: "memory"); }
-__device__ __forceinline__ void p8_await_selects() { asm volatile("bar.sync 2, 416;" ::: "memory"); }
+__device__ __forceinline__ void p8_signal_selects(int site) { jit_point(site); asm volatile("bar.arrive 2, 416;" ::: "memory"); }
+__device__ __forceinline__ void p8_await_selects(int site) { asm volatile("bar.sync 2, 416;" ::: "memory"); jit_point(site); }
 // named barrier 1 (warps 0-11): behind lane 0's numbering of a clashing bit and behind the apply phase, before lane 0's
 // epilogue reads res2 and clash; on the bit that starts a byte also between the probe and the numbering. Inside a byte the
 // unit warps 13-15 are not in it (nothing behind it reads their inputs before the bit's last __syncthreads)
-__device__ __forceinline__ void p8_sync_maps() { asm volatile("bar.sync 1, 384;" ::: "memory"); static_assert(P8_MAP_THREADS == 384, "named barrier width"); }
+__device__ __forceinline__ void p8_sync_maps(int site) { asm volatile("bar.sync 1, 384;" ::: "memory"); jit_point(site); static_assert(P8_MAP_THREADS == 384, "named barrier width"); }
 // The bit that starts a byte runs its context computation as independent chains of warps (p8_model_bit) ordered by three
 // more named barriers. Every arrive / sync below is executed by whole warps, unconditionally on that bit:
 //  3 (join, 480): "the new contexts of every map are set". Warps 0-11 sync on it before the probe of the 7-slot maps
@@ -634,10 +635,10 @@ __device__ __forceinline__ void p8_sync_maps() { asm volatile("bar.sync 1, 384;"
 //  5 (96):        the text chain's warps 13-15 between its steps.
 // Inside a byte barrier 3 is the probe / apply boundary, with the same warps: all of them sync (the unit warps 13-15 apply
 // what warps 9-11 probed and the reverse).
-__device__ __forceinline__ void p8_join_sync() { asm volatile("bar.sync 3, 480;" ::: "memory"); }
-__device__ __forceinline__ void p8_join_arrive() { __threadfence_block(); asm volatile("bar.arrive 3, 480;" ::: "memory"); }
-__device__ __forceinline__ void p8_sync_dchain() { asm volatile("bar.sync 4, 160;" ::: "memory"); }
-__device__ __forceinline__ void p8_sync_text() { asm volatile("bar.sync 5, 96;" ::: "memory"); }
+__device__ __forceinline__ void p8_join_sync(int site) { asm volatile("bar.sync 3, 480;" ::: "memory"); jit_point(site); }
+__device__ __forceinline__ void p8_join_arrive(int site) { jit_point(site); __threadfence_block(); asm volatile("bar.arrive 3, 480;" ::: "memory"); }
+__device__ __forceinline__ void p8_sync_dchain(int site) { asm volatile("bar.sync 4, 160;" ::: "memory"); jit_point(site); }
+__device__ __forceinline__ void p8_sync_text(int site) { asm volatile("bar.sync 5, 96;" ::: "memory"); jit_point(site); }
 enum { P8_WARP_D = P8_CM2_TID0 / 32, P8_WARP_TEXT = P8_MAP_WARPS + 1 };   // first warp of the D-chain / of the text chain
 static_assert(P8_CM2_TID0 % 32 == 0 && P8_CM_LANES <= P8_CM2_TID0 && (P8_MAP_WARPS - P8_WARP_D) * 32 == 160, "barrier 4: warps 7-11");
 static_assert((P8_WARPS - P8_WARP_TEXT) * 32 == 96 && P8_MAP_THREADS + 96 == 480, "barriers 3 and 5: warps 13-15 beside the 12 map warps");
@@ -652,16 +653,18 @@ __device__ __forceinline__ u32 p8_smem(const void* p) { return (u32)__cvta_gener
 __device__ __forceinline__ void p8_mbar_init(unsigned long long* b, int count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(p8_smem(b)), "r"(count) : "memory");
 }
-__device__ __forceinline__ void p8_mbar_arrive_remote(unsigned long long* b, int rank) {
+__device__ __forceinline__ void p8_mbar_arrive_remote(unsigned long long* b, int rank, int site) {
+  jit_point(site);
   u32 r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(p8_smem(b)), "r"(rank));
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(r) : "memory");
 }
-__device__ __forceinline__ void p8_mbar_wait(unsigned long long* b, u32 parity) {
+__device__ __forceinline__ void p8_mbar_wait(unsigned long long* b, u32 parity, int site) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "P8W: mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
       "@!p bra P8W;\n\t}" ::"r"(p8_smem(b)), "r"(parity) : "memory");
+  jit_point(site);
 }
 
 // Mixer::update for the 28 cached weight sets selected for the previous bit, on its inputs tx (all lanes of the mixer CTA)
@@ -733,13 +736,13 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     for (int k = tid; k < P8_SEEN; k += P8_THREADS) sh.u.md.seen[k] = 0ull;
     if (tid == 0) P8_U(22);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   P8_T(0);
   const int bpos = S.bpos, c0 = S.c0;
   const bool byte_start = bpos == 0;
   if (tid >= P8_MAP_THREADS) {
     if (warp == P8_MAP_WARPS) {            // ModelStats and the 19 selector sets that do not wait for the order-N map
-      p8_await_selects();
+      p8_await_selects(JIT_HERE);
       if (lane == 0) {
         xml_stats(S);
         smatch_select(S);
@@ -754,12 +757,12 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       // each, then the 33 contexts side by side. Nothing else reads the text model before the join.
       P8_M0;
       if (tid == P8_WARP_TEXT * 32) sh.text_pending = text_update_a(S);
-      p8_sync_text();
+      p8_sync_text(JIT_HERE);
       if (sh.text_pending) {
         const int split = S.text.stem_split;
         const int i = warp == P8_WARP_TEXT ? LANG_EN : (warp == P8_WARP_TEXT + 1 ? LANG_FR : LANG_DE);
         if (lane == 0 && i >= split) text_stem(S, i);
-        p8_sync_text();
+        p8_sync_text(JIT_HERE);
         if (tid == P8_WARP_TEXT * 32) {
           text_stem_mid(S);
           for (int j = split - 1; j > LANG_UNKNOWN; --j) text_stem(S, j);
@@ -772,7 +775,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         __syncwarp();
         if (lane == 0) { S.text.map.index = n; P8_M(38); }
       }
-      p8_join_arrive();
+      p8_join_arrive(JIT_HERE);
     } else {
       // ---- inside a byte, warps 13-15: single-lane units beside the maps; the apply runs while lane 0 numbers a clashing bit
       {
@@ -781,7 +784,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         __syncwarp();
         if (lane == 0) P8_M(24 + warp);
       }
-      p8_join_sync();
+      p8_join_sync(JIT_HERE);
       {
         P8_M0;
         p8_apply_units(sh, warp, lane, y, c0, bpos);
@@ -800,14 +803,14 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
           // models, which consume the order-N map's result and the match length of this bit
           if (tid == P8_CM2_TID0) ordern_byte(S);
           else if (tid == P8_TID_MATCH) exe_byte(S);
-          p8_sync_dchain();
+          p8_sync_dchain(JIT_HERE);
           if (tid == P8_CM2_TID0) P8_M(31);
           p8_probe_cm2(sh, tid, bpos, 5);
           p8_probe_single(sh, tid, y, c0, bpos);
-          p8_sync_dchain();
+          p8_sync_dchain(JIT_HERE);
           if (tid == P8_CM2_TID0) P8_M(32);
           p8_apply_cm2(sh, tid, y, bpos, 5);
-          p8_sync_dchain();
+          p8_sync_dchain(JIT_HERE);
           if (tid == P8_CM2_TID0) P8_M(33);
           const int ismatch = ilog(T, S.match.length);
           if (tid == P8_TID_MATCH) { sparse_byte(S, ismatch, sh.res2[0]); P8_M(34); }
@@ -837,20 +840,20 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         }
         if (lane == 0 && warp < P8_WARP_D) P8_M(24 + warp);
       }
-      p8_join_sync();
-      p8_signal_selects();
+      p8_join_sync(JIT_HERE);
+      p8_signal_selects(JIT_HERE);
       P8_T(2);
       // ---- the sixteen 7-slot maps in one probe / number / apply (their random draws are shared), the text history map beside them
       if (warp < P8_WARP_D) p8_probe_cm(sh, tid, y, c0, bpos);
       else p8_probe_cm2(sh, tid, bpos, 2);
-      p8_sync_maps();
+      p8_sync_maps(JIT_HERE);
       P8_T(6);
-      if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(); }
+      if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(JIT_HERE); }
       P8_T(7);
       p8_apply_cm(sh, tid, y, c0, bpos);
       p8_apply_cm2(sh, tid, y, bpos, 2);
       p8_apply_small(sh, tid, y, bpos);
-      p8_sync_maps();
+      p8_sync_maps(JIT_HERE);
       P8_T(8);
     } else {
       // ---- inside a byte: probe / number / apply, all map families side by side, the single-lane units on warps 9-11 and
@@ -863,10 +866,10 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         __syncwarp();
         if (lane == 0) P8_M(24 + warp);
       }
-      p8_join_sync();
-      p8_signal_selects();
+      p8_join_sync(JIT_HERE);
+      p8_signal_selects(JIT_HERE);
       P8_T(3);
-      if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(); }
+      if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(JIT_HERE); }
       P8_T(7);
       {
         P8_M0;
@@ -876,7 +879,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         __syncwarp();
         if (lane == 0) P8_M(48 + warp);
       }
-      p8_sync_maps();
+      p8_sync_maps(JIT_HERE);
       P8_T(8);
     }
     // ---- epilogues, ModelStats, the 28 selector sets in the reference's order
@@ -897,12 +900,12 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
 #endif
     }
   }
-  __syncthreads();     // warp 12 joins
+  JIT_SYNCTHREADS();     // warp 12 joins
   P8_T(9);
   // ---- hand the bit over. Only warp 0 reads the scalars: its lane 0 is the one that changes them at the next bit's start,
   // the other warps' data (inputs, codes) changes only after the next bit's first barrier.
   const int slot = (int)(t % P8_RING);
-  if (t >= P8_RING) p8_mbar_wait(&sh.empty[slot], (t / P8_RING - 1) & 1);
+  if (t >= P8_RING) p8_mbar_wait(&sh.empty[slot], (t / P8_RING - 1) & 1, JIT_HERE);
   P8_T(10);
   {
     const Mixer& m = S.m;
@@ -918,7 +921,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     for (int q = tid; q < m.nx / 8; q += P8_THREADS) reinterpret_cast<uint4*>(d.tx)[q] = reinterpret_cast<const uint4*>(m.tx)[q];
     for (int q = tid; q < (m.n2 + 1) / 2; q += P8_THREADS) reinterpret_cast<u32*>(d.codes)[q] = reinterpret_cast<const u32*>(S.codes)[q];
     __syncwarp();
-    if (lane == 0) p8_mbar_arrive_remote(&sh.full[slot], 1);
+    if (lane == 0) p8_mbar_arrive_remote(&sh.full[slot], 1, JIT_HERE);
   }
   P8_T(11);
 #ifdef P8_PROF
@@ -959,12 +962,12 @@ __device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_p
   }
   P8_T(17);
   // ---- the bit's inputs and selectors (set 26 from this CTA's last prediction)
-  p8_mbar_wait(&sh.full[slot], (t / P8_RING) & 1);
+  p8_mbar_wait(&sh.full[slot], (t / P8_RING) & 1, JIT_HERE);
   P8_T(16);
   if (tid < N_SETS) m.cxt[tid] = tid == MAIN_SET_FIRST + 7 ? MAIN_SET_PR + S.last_prediction / 16 : in.cxt[tid];
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) {
-    if (t > 0) p8_mbar_arrive_remote(&sh.empty[(t - 1) % P8_RING], 0);   // tx_prev was slot t-1's
+    if (t > 0) p8_mbar_arrive_remote(&sh.empty[(t - 1) % P8_RING], 0, JIT_HERE);   // tx_prev was slot t-1's
     S.st_misses += S.st_misses + (u64)((S.pr >> 11) != y);               // bit_begin's line, on this CTA's prediction
     S.y = y; S.c0 = in.c0; S.bpos = in.bpos; S.blpos = in.blpos; S.c4 = in.c4; S.st_type = in.st_type;
     S.st_match_length = in.st_match_length; S.st_match_expected = in.st_match_expected;
@@ -1002,7 +1005,7 @@ __device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_p
       if (lane == 0) sh.dot[i] = acc;
     }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   P8_T(18);
   // ---- squash, final mixer, SSE stage (one warp)
   if (warp == 0) {
@@ -1023,14 +1026,14 @@ __device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_p
     __syncwarp();
     p8_sse_warp(sh, pr2, in.c1, lane);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   P8_T(19);
 }
 
 // Both CTAs: state block and hot tables into shared memory, the ring's barriers; the mixer CTA: the pending weight sets.
 __device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g, int tid, int rank) {
   p8_copy_words(&sh.S, g, sizeof(p8::State), tid);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   const p8::Tables* gT = sh.S.T;
   p8_copy_words(sh.tab, gT, p8::TABLES_HOT_BYTES, tid);
   if (tid < p8::N_SETS) sh.wc_set[tid] = -1;
@@ -1044,7 +1047,7 @@ __device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) sh.S.T = reinterpret_cast<const p8::Tables*>(sh.tab);
   const int warp = tid >> 5, lane = tid & 31;
   if (rank == 1) {
@@ -1053,7 +1056,7 @@ __device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g
       if (lane == 0) sh.wc_set[i] = sh.S.m.cxt[i];
     }
   }
-  cooperative_groups::this_cluster().sync();   // the barriers exist before the other CTA arrives on them
+  jit_cluster_sync(cooperative_groups::this_cluster(), JIT_HERE);   // the barriers exist before the other CTA arrives on them
   return gT;
 }
 // Each CTA writes back the fields it owns: the mixer CTA `m`, the APMs and `codes` (with the inputs of the last bit it
@@ -1068,14 +1071,14 @@ __device__ __forceinline__ void p8_leave(P8Shared& sh, p8::State* g, const p8::T
       if (sh.wc_set[i] >= 0) p8_row_store(sh.S.m.w + (size_t)sh.wc_set[i] * N_IN, sh.u.mx.wc[i], lane);
     if (last >= 0) for (int q = tid; q < sh.S.m.nx / 8; q += P8_THREADS) reinterpret_cast<uint4*>(sh.S.m.tx)[q] = reinterpret_cast<const uint4*>(sh.u.mx.ring[last].tx)[q];
   }
-  cluster.sync();
+  jit_cluster_sync(cluster, JIT_HERE);
   if (rank == 0 && tid == 0) {
     const State& X = cluster.map_shared_rank(&sh, 1)->S;
     sh.S.pr = X.pr; sh.S.last_prediction = X.last_prediction; sh.S.st_misses = X.st_misses;
     sh.S.error |= X.error;
     sh.S.T = gT;
   }
-  cluster.sync();   // the mixer CTA's shared memory stays until the model CTA has read it
+  jit_cluster_sync(cluster, JIT_HERE);   // the mixer CTA's shared memory stays until the model CTA has read it
   const size_t m0 = offsetof(State, m), e0 = offsetof(State, error);
   static_assert(offsetof(State, m) % 4 == 0 && offsetof(State, error) % 4 == 0, "state block is copied word by word");
   if (rank == 0) {
@@ -1087,7 +1090,7 @@ __device__ __forceinline__ void p8_leave(P8Shared& sh, p8::State* g, const p8::T
 }
 
 // Bulk: cluster b (CTAs 2b, 2b+1) serves stream b of the launch group: writes ext[t][431..2021] for every bit t of the sub-chunk.
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P8_THREADS, 1) paq8_kernel(const ChunkArgs* __restrict__ args_all) {
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P8_THREADS, 1) paq8_kernel(const ChunkArgs* __restrict__ args_all) { jit_entry(JK_PAQ8);
   extern __shared__ __align__(16) unsigned char p8_raw[];
   P8Shared& sh = *reinterpret_cast<P8Shared*>(p8_raw);
   const ChunkArgs a = args_all[blockIdx.x >> 1];
@@ -1117,7 +1120,7 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P8_THREADS, 1) paq8_
 }
 
 // Lock-step: one bit per launch, a one-slot handover; the codes for the next Predict() land in ext_bit[431..2021].
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P8_THREADS, 1) paq8_bit_kernel(p8::State* g, int y, u16* ext_bit, const u32* dbit) {
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P8_THREADS, 1) paq8_bit_kernel(p8::State* g, int y, u16* ext_bit, const u32* dbit) { jit_entry(JK_PAQ8_BIT);
   if (dbit) y = (int)dbit[0];
   extern __shared__ __align__(16) unsigned char p8_raw[];
   P8Shared& sh = *reinterpret_cast<P8Shared*>(p8_raw);

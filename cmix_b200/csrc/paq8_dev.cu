@@ -16,6 +16,10 @@ void paq8_launch_bit(p8::State* g, int y, u16* ext_bit, cudaStream_t s, const u3
   paq8_bit_kernel<<<2, P8_THREADS, sizeof(P8Shared), s>>>(g, y, ext_bit, dbit);
 }
 
+#ifdef CMIXB200_JITTER
+JIT_MODULE(paq8)
+#endif
+
 }  // namespace cmixb200
 
 #ifdef P8_PROF

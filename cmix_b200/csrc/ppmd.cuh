@@ -10,6 +10,7 @@
 // stream, one warp per stream, all warps of a launch group in one CTA.
 #pragma once
 #include "exact_math.h"
+#include "jitter.cuh"
 #include "ppmd_model.h"
 #include "state.h"
 
@@ -155,7 +156,7 @@ __device__ void ppmd_prepare_byte_warp(PpmdModel& m, int lane) {
   __syncwarp();
 }
 
-__global__ void ppmd_init_kernel(PpmdModel* m) {
+__global__ void ppmd_init_kernel(PpmdModel* m) { jit_entry(JK_PPMD_INIT);
   if (threadIdx.x == 0 && blockIdx.x == 0) ppmd_init(*m);
 }
 
@@ -174,7 +175,7 @@ __device__ __forceinline__ void ppmd_copy_words(void* dst, const void* src, int 
 struct PpmdWarpShared { PpmdModel m; float scratch[256]; };
 
 // Bulk: warp w of block b serves stream b * PPMD_WARPS + w of the launch group.
-__global__ void __launch_bounds__(PPMD_WARPS * 32, 1) ppmd_kernel(const ChunkArgs* __restrict__ args_all, int n_streams) {
+__global__ void __launch_bounds__(PPMD_WARPS * 32, 1) ppmd_kernel(const ChunkArgs* __restrict__ args_all, int n_streams) { jit_entry(JK_PPMD);
   extern __shared__ __align__(16) unsigned char ppmd_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   PpmdWarpShared& sh = reinterpret_cast<PpmdWarpShared*>(ppmd_raw)[warp];
@@ -199,7 +200,7 @@ __global__ void __launch_bounds__(PPMD_WARPS * 32, 1) ppmd_kernel(const ChunkArg
 }
 
 // Lock-step: one byte.
-__global__ void __launch_bounds__(32, 1) ppmd_byte_kernel(StreamState* st, u32 byte, float* out, const u32* dbit = nullptr) {
+__global__ void __launch_bounds__(32, 1) ppmd_byte_kernel(StreamState* st, u32 byte, float* out, const u32* dbit = nullptr) { jit_entry(JK_PPMD_BYTE);
   if (dbit) byte = dbit[1];
   extern __shared__ __align__(16) unsigned char ppmd_raw[];
   PpmdWarpShared& sh = *reinterpret_cast<PpmdWarpShared*>(ppmd_raw);

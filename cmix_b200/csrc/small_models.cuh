@@ -13,6 +13,7 @@
 // their dependent HBM loads concurrently instead of one after the other.
 #pragma once
 #include "exact_math.h"
+#include "jitter.cuh"
 #include "state.h"
 #include "bytemodel.cuh"
 
@@ -315,7 +316,7 @@ __device__ void bracket_byte_update(SmallState& s, float* probs, u32 byte, int t
     s.bk_depth = depth;
     *sh_p = p; *sh_hot = hot;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   const float p = *sh_p; const int hot = *sh_hot;
   const float rest = p < 0.0f ? (float)(1. / 256) : XM_FDIV(XM_FSUB(1.0f, p), 255.0f);
   for (int i = tid; i < 256; i += nthreads) {
@@ -323,7 +324,7 @@ __device__ void bracket_byte_update(SmallState& s, float* probs, u32 byte, int t
     if (!s.vocab[i]) v = 0.0f;                       // ByteModel::ByteUpdate (byte-model.cpp:39-45)
     probs[i] = v;
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
 }
 
 // One bit of Predict() for the small models: writes 54 stretched inputs + PPMD input + selectors.
@@ -369,13 +370,13 @@ __device__ void small_perceive(SmallState& s, SmallShared& sh, int bit, const fl
   // are serialised in model order.
   sh.ind_addr[tid] = my_addr;
   if (tid == 0) sh.max_rank = 0;
-  __syncthreads();
+  JIT_SYNCTHREADS();
   int rank = 0;
   if (r.kind == K_INDIRECT) {
     for (int l = 0; l < tid; ++l) if (sh.ind_addr[l] == my_addr) ++rank;
     if (rank) atomicMax(&sh.max_rank, rank);
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   const int max_rank = sh.max_rank;
   for (int pass = 0; pass <= max_rank; ++pass) {
     if (r.kind == K_INDIRECT && rank == pass) {
@@ -386,20 +387,20 @@ __device__ void small_perceive(SmallState& s, SmallShared& sh, int bit, const fl
       s.shared_map[m.map_index] = m.run ? c_runmap[state * 2 + bit] : c_nonstat[state * 2 + bit];
       m.map_index -= bc;
     }
-    if (max_rank) { __threadfence_block(); __syncthreads(); }
+    if (max_rank) { __threadfence_block(); JIT_SYNCTHREADS(); }
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   // --- ContextManager::UpdateContexts ---
   const bool byte_update = bc >= 128;
   const u32 full = (bc * 2 + bit) & 255;          // the byte just completed (valid if byte_update)
   if (tid == 0) contexts_update(s, bit);
   if (byte_update && tid >= 32 && tid < 43) ihash_update(s.ihash[tid - 32], full);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (tid == 0) { bitcontexts_update(s); sh.longest_match = 0; }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   if (byte_update) {
     if (tid == 0) small_refresh_tables(s, sh);   // new byte-level context values for ByteUpdate()
-    __syncthreads();
+    JIT_SYNCTHREADS();
     // --- Model::ByteUpdate (bit_context_ still holds the full byte, quirk 14) ---
     switch (r.kind) {
       case K_DHASH: dhash_byte_update(r.idx == 0 ? s.dhash_word : s.dhash_o3, sh.ctxv[r.ctx]); break;
@@ -414,17 +415,17 @@ __device__ void small_perceive(SmallState& s, SmallShared& sh, int bit, const fl
       // no replayed PPMD stream: the slot carries a flat distribution over the vocabulary
       sh.ppmd_probs[i] = ppmd_next ? ppmd_next[i] : (s.vocab[i] ? (float)(1. / 256) : 0.0f);
     }
-    __syncthreads();
+    JIT_SYNCTHREADS();
     if (tid == 0) {
       s.bracket_bm.top = 255; s.bracket_bm.bot = 0;
       if (!pretrain) { s.ppmd_bm.top = 255; s.ppmd_bm.bot = 0; }
       s.longest_match = sh.longest_match;
       s.bit_context = 1;                           // predictor.cpp:468
     }
-    __syncthreads();
+    JIT_SYNCTHREADS();
   }
   if (tid == 0) small_refresh_tables(s, sh);
-  __syncthreads();
+  JIT_SYNCTHREADS();
 }
 
 // Bulk kernel: all bits of a chunk (compress direction: the bits are known).
@@ -432,7 +433,7 @@ __device__ void small_perceive(SmallState& s, SmallShared& sh, int bit, const fl
 // the big HBM tables) lives in shared memory for the duration of the kernel: a state machine that
 // chases `state->table_ptr` through HBM pays ~1 us per dependent load; out of shared memory it pays 30 ns.
 __global__ void __launch_bounds__(64, 1)
-small_kernel(const ChunkArgs* __restrict__ args_all, Tables T) {
+small_kernel(const ChunkArgs* __restrict__ args_all, Tables T) { jit_entry(JK_SMALL);
   const ChunkArgs a = args_all[blockIdx.x];
   StreamState* st = a.st;
   extern __shared__ __align__(16) unsigned char small_raw[];
@@ -444,10 +445,10 @@ small_kernel(const ChunkArgs* __restrict__ args_all, Tables T) {
     uint4* dst = reinterpret_cast<uint4*>(small_raw);
     for (int i = tid; i < (int)(sizeof(SmallState) / 16); i += 64) dst[i] = src[i];
   }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   for (int i = tid; i < 256; i += 64) { sh.bracket_probs[i] = s.bracket_bm.probs[i]; sh.ppmd_probs[i] = s.ppmd_bm.probs[i]; }
   if (tid == 0) small_refresh_tables(s, sh);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   for (u32 pos = 0; pos < a.n_bytes; ++pos) {
     const u32 byte = a.bytes[pos];
     for (int j = 7; j >= 0; --j) {
@@ -455,12 +456,12 @@ small_kernel(const ChunkArgs* __restrict__ args_all, Tables T) {
       const int bit = (byte >> j) & 1;
       small_predict(s, T, sh, a.pretrain ? st->small_x : a.small_x + t * SMALL_X_PITCH,
                     a.pretrain ? st->sel : a.sel + t * SEL_PITCH, tid);
-      __syncthreads();
+      JIT_SYNCTHREADS();
       small_perceive(s, sh, bit, (j == 0 && a.ppmd) ? a.ppmd + (u64)pos * 256 : nullptr, (int)a.pretrain, tid, 64);
     }
   }
   for (int i = tid; i < 256; i += 64) { s.bracket_bm.probs[i] = sh.bracket_probs[i]; s.ppmd_bm.probs[i] = sh.ppmd_probs[i]; }
-  __syncthreads();
+  JIT_SYNCTHREADS();
   {
     uint4* dst = reinterpret_cast<uint4*>(&st->small);
     const uint4* src = reinterpret_cast<const uint4*>(small_raw);
@@ -469,23 +470,23 @@ small_kernel(const ChunkArgs* __restrict__ args_all, Tables T) {
 }
 
 // Lock-step halves (Predictor::Predict / Perceive called bit by bit from the host).
-__global__ void __launch_bounds__(64, 1) small_predict_kernel(StreamState* st, Tables T) {
+__global__ void __launch_bounds__(64, 1) small_predict_kernel(StreamState* st, Tables T) { jit_entry(JK_SMALL_PREDICT);
   __shared__ SmallShared sh;
   SmallState& s = st->small;
   const int tid = threadIdx.x;
   for (int i = tid; i < 256; i += 64) { sh.bracket_probs[i] = s.bracket_bm.probs[i]; sh.ppmd_probs[i] = s.ppmd_bm.probs[i]; }
   if (tid == 0) small_refresh_tables(s, sh);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   small_predict(st->small, T, sh, st->small_x, st->sel, tid);
 }
-__global__ void __launch_bounds__(64, 1) small_perceive_kernel(StreamState* st, int bit, const float* ppmd_next, int pretrain, const u32* dbit = nullptr) {
+__global__ void __launch_bounds__(64, 1) small_perceive_kernel(StreamState* st, int bit, const float* ppmd_next, int pretrain, const u32* dbit = nullptr) { jit_entry(JK_SMALL_PERCEIVE);
   if (dbit) bit = (int)dbit[0];
   __shared__ SmallShared sh;
   SmallState& s = st->small;
   const int tid = threadIdx.x;
   for (int i = tid; i < 256; i += 64) { sh.bracket_probs[i] = s.bracket_bm.probs[i]; sh.ppmd_probs[i] = s.ppmd_bm.probs[i]; }
   if (tid == 0) small_refresh_tables(s, sh);
-  __syncthreads();
+  JIT_SYNCTHREADS();
   small_perceive(st->small, sh, bit, ppmd_next, pretrain, tid, 64);
   for (int i = tid; i < 256; i += 64) { s.bracket_bm.probs[i] = sh.bracket_probs[i]; s.ppmd_bm.probs[i] = sh.ppmd_probs[i]; }
 }
