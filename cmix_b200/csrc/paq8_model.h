@@ -33,6 +33,10 @@
 #ifndef P8_CENSUS_CM2
 #define P8_CENSUS_CM2(m, bpos) do { } while (0)
 #endif
+// Profiling build of the device (paq8.cuh with -DP8_PROF): the end of leg k of a 7-slot map context's bit. Empty elsewhere.
+#ifndef P8_LEG
+#define P8_LEG(k) do { } while (0)
+#endif
 
 namespace cmixb200 {
 namespace p8 {
@@ -360,7 +364,7 @@ P8_HD inline int cm_step(Cm& m, int i, Out& o, int ns, int y, int c0, int bp, in
       } break;
     }
   }
-  if ((bp == 1 || bp == 4) && m.cp[i] != P8_NULL) bucket_prefetch2(t, m.mask, m.cxt[i], (u32)c0 * 2);
+  if ((bp == 1 || bp == 4) && m.cp[i] != P8_NULL) bucket_prefetch2(t, m.mask, m.cxt[i], (u32)c0 * 2); P8_LEG(4);
   const u8* rp = t + m.runp[i];
   const int rc = rp[0];
   if (((rp[1] + 256) >> (8 - bp)) == c0) {
@@ -368,7 +372,7 @@ P8_HD inline int cm_step(Cm& m, int i, Out& o, int ns, int y, int c0, int bp, in
     const int c = ilog(T, rc + 1) << (2 + (~rc & 1));
     add(o, b * c);
   } else add(o, 0);
-  const int s = m.cp[i] != P8_NULL ? t[m.cp[i]] : 0;
+  P8_LEG(5); const int s = m.cp[i] != P8_NULL ? t[m.cp[i]] : 0;
   u16 fresh = smt[s];
   const u16 upd = (u16)(sm_old + (((y << 16) - (int)sm_old + 128) >> 8));   // StateMap16 update of the previous bit's cell
   if (s == so) fresh = upd;
@@ -376,12 +380,12 @@ P8_HD inline int cm_step(Cm& m, int i, Out& o, int ns, int y, int c0, int bp, in
   m.sm_cxt[i] = s;
   const int p1 = fresh >> 4;
   const int st = (stretch(T, p1) + 2) >> 2;
-  add(o, st);
+  add(o, st); P8_LEG(6);
   add(o, (p1 - 2047 + 4) >> 3);
   const int n0 = -!T.state[s][2], n1 = -!T.state[s][3];
   add(o, st * iabs(n1 - n0));
   const int p0 = 4095 - p1;
-  add(o, ((p1 & n0) - (p0 & n1) + 8) >> 4);
+  add(o, ((p1 & n0) - (p0 & n1) + 8) >> 4); P8_LEG(7);
   return s > 0;
 }
 // The in-order loop. `rnd` is the global generator: draws happen in context order.

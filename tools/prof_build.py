@@ -45,6 +45,11 @@ P8_UNITS = {
     23: "lane 0: epilogue (main_select_fixed, padding)",
 }
 P8_LABELS.update({64 + g: "unit: " + s for g, s in P8_UNITS.items()})
+# 88 + k: leg k of a 7-slot map context's bit, the longest lane of the bit (each leg apart)
+P8_LEGS = ["probe: state read", "probe: touched_buckets", "probe: p8_claim", "apply: draw",
+           "apply: store and move (bucket_find at bpos 2, 5, 0)", "apply: run record input", "apply: cell state and StateMap load",
+           "apply: other exports"]
+P8_LABELS.update({88 + k: "7-slot lane leg: " + s for k, s in enumerate(P8_LEGS)})
 P8_ROWS, P8_SLOTS = 6, 128
 P8_CLASSES = ["byte boundary", "inside a byte", "same bucket", "same bucket, clash", "new bucket", "new bucket, clash"]
 
