@@ -10,10 +10,10 @@ cudaError_t fxcm_configure() {
   return cudaFuncSetAttribute(fxcm_bit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FxShared));
 }
 void fxcm_launch_chunk(const ChunkArgs* d_args, int n_streams, cudaStream_t s) {
-  fxcm_kernel<<<n_streams, FX_THREADS, sizeof(FxShared), s>>>(d_args);
+  fxcm_kernel<<<2 * n_streams, FX_THREADS, sizeof(FxShared), s>>>(d_args);
 }
 void fxcm_launch_bit(StreamState* st, fx::State* g, int y, int pretrain, u16* ext_bit, cudaStream_t s, const u32* dbit) {
-  fxcm_bit_kernel<<<1, FX_THREADS, sizeof(FxShared), s>>>(st, g, y, pretrain, ext_bit, dbit);
+  fxcm_bit_kernel<<<2, FX_THREADS, sizeof(FxShared), s>>>(st, g, y, pretrain, ext_bit, dbit);
 }
 
 #ifdef CMIXB200_JITTER

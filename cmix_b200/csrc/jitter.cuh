@@ -33,7 +33,8 @@ enum { JG_NONE,
        JG_P8_OLS, JG_P8_W3_6, JG_P8_DCHAIN, JG_P8_W12, JG_P8_W13_15, JG_P8_MIXER,   // PAQ8: model CTA warps, mixer CTA
        JG_MIX_C, JG_MIX_T, JG_MIX_MOVERS, JG_MIX_CTA1,                            // mix_kernel_v3: CTA 0's roles, CTA 1
        JG_LSTM_R0, JG_LSTM_R1, JG_LSTM_R2, JG_LSTM_R3, JG_LSTM_R4, JG_LSTM_R5, JG_LSTM_R6, JG_LSTM_R7,   // the LSTM cluster, by rank
-       JG_FXCM, JG_PPMD, JG_SMALL, JG_MIX_LOCK, JG_CODER, JG_ENGINE, JIT_N_GROUPS };
+       JG_FX_MODEL, JG_FX_MIXER,                                                    // FXCM: model CTA, mixer CTA
+       JG_PPMD, JG_SMALL, JG_MIX_LOCK, JG_CODER, JG_ENGINE, JIT_N_GROUPS };
 enum { JIT_OFF, JIT_RANDOM, JIT_STARVE, JIT_HURRY, JIT_ENTRY };
 
 #ifdef CMIXB200_JITTER
@@ -70,7 +71,7 @@ __device__ __forceinline__ int jit_group(int file, int rank, int warp) {
     case JF_PAQ8: return rank == 1 ? JG_P8_MIXER : warp < 3 ? JG_P8_OLS : warp < 7 ? JG_P8_W3_6 : warp < 12 ? JG_P8_DCHAIN : warp == 12 ? JG_P8_W12 : JG_P8_W13_15;
     case JF_MIX_BULK: return rank == 1 ? JG_MIX_CTA1 : warp == 15 ? JG_MIX_C : warp == 14 ? JG_MIX_T : (warp & 3) != 3 ? JG_MIX_MOVERS : JG_NONE;
     case JF_LSTM: return JG_LSTM_R0 + (rank & 7);
-    case JF_FXCM: return JG_FXCM;
+    case JF_FXCM: return rank == 1 ? JG_FX_MIXER : JG_FX_MODEL;
     case JF_PPMD: return JG_PPMD;
     case JF_SMALL: return JG_SMALL;
     case JF_MIX_LOCK: return JG_MIX_LOCK;

@@ -37,6 +37,7 @@
 #pragma once
 #include <cooperative_groups.h>
 #include "jitter.cuh"
+#include "cluster_mbar.cuh"
 #ifdef P8_PROF
 namespace cmixb200 { __host__ __device__ inline void p8_leg(int k); }
 #define P8_LEG(k) ::cmixb200::p8_leg(k)
@@ -678,26 +679,6 @@ static_assert(P8_W_MATCH > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_SM
               P8_W_IMAP > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_DMCMIX < (int)P8_MAP_WARPS && (int)P8_W_SM32 == (int)P8_WARP_TEXT && (int)P8_W_STM == (int)P8_WARPS - 1,
               "barrier 3 inside a byte: the unit warps are 9-11 (in barriers 1 and 2 with the map warps) and 13-15 (in barrier 3 only)");
 
-// The ring's mbarriers. An arrive on the other CTA's barrier releases at cluster scope what the arriving thread wrote or
-// read before it; a wait acquires it.
-__device__ __forceinline__ u32 p8_smem(const void* p) { return (u32)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void p8_mbar_init(unsigned long long* b, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(p8_smem(b)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void p8_mbar_arrive_remote(unsigned long long* b, int rank, int site) {
-  jit_point(site);
-  u32 r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(p8_smem(b)), "r"(rank));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(r) : "memory");
-}
-__device__ __forceinline__ void p8_mbar_wait(unsigned long long* b, u32 parity, int site) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "P8W: mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
-      "@!p bra P8W;\n\t}" ::"r"(p8_smem(b)), "r"(parity) : "memory");
-  jit_point(site);
-}
-
 // Mixer::update for the 28 cached weight sets selected for the previous bit, on its inputs tx (all lanes of the mixer CTA)
 __device__ __forceinline__ void p8_sgd(P8Shared& sh, const short* tx, int y, int tid) {
   using namespace p8;
@@ -936,7 +917,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
   // ---- hand the bit over. Only warp 0 reads the scalars: its lane 0 is the one that changes them at the next bit's start,
   // the other warps' data (inputs, codes) changes only after the next bit's first barrier.
   const int slot = (int)(t % P8_RING);
-  if (t >= P8_RING) p8_mbar_wait(&sh.empty[slot], (t / P8_RING - 1) & 1, JIT_HERE);
+  if (t >= P8_RING) mbar_wait(&sh.empty[slot], (t / P8_RING - 1) & 1, JIT_HERE);
   P8_T(10);
   {
     const Mixer& m = S.m;
@@ -952,7 +933,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     for (int q = tid; q < m.nx / 8; q += P8_THREADS) reinterpret_cast<uint4*>(d.tx)[q] = reinterpret_cast<const uint4*>(m.tx)[q];
     for (int q = tid; q < (m.n2 + 1) / 2; q += P8_THREADS) reinterpret_cast<u32*>(d.codes)[q] = reinterpret_cast<const u32*>(S.codes)[q];
     __syncwarp();
-    if (lane == 0) p8_mbar_arrive_remote(&sh.full[slot], 1, JIT_HERE);
+    if (lane == 0) mbar_arrive_remote(&sh.full[slot], 1, JIT_HERE);
   }
   P8_T(11);
 #ifdef P8_PROF
@@ -993,12 +974,12 @@ __device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_p
   }
   P8_T(17);
   // ---- the bit's inputs and selectors (set 26 from this CTA's last prediction)
-  p8_mbar_wait(&sh.full[slot], (t / P8_RING) & 1, JIT_HERE);
+  mbar_wait(&sh.full[slot], (t / P8_RING) & 1, JIT_HERE);
   P8_T(16);
   if (tid < N_SETS) m.cxt[tid] = tid == MAIN_SET_FIRST + 7 ? MAIN_SET_PR + S.last_prediction / 16 : in.cxt[tid];
   JIT_SYNCTHREADS();
   if (tid == 0) {
-    if (t > 0) p8_mbar_arrive_remote(&sh.empty[(t - 1) % P8_RING], 0, JIT_HERE);   // tx_prev was slot t-1's
+    if (t > 0) mbar_arrive_remote(&sh.empty[(t - 1) % P8_RING], 0, JIT_HERE);   // tx_prev was slot t-1's
     S.st_misses += S.st_misses + (u64)((S.pr >> 11) != y);               // bit_begin's line, on this CTA's prediction
     S.y = y; S.c0 = in.c0; S.bpos = in.bpos; S.blpos = in.blpos; S.c4 = in.c4; S.st_type = in.st_type;
     S.st_match_length = in.st_match_length; S.st_match_expected = in.st_match_expected;
@@ -1073,8 +1054,8 @@ __device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g
 #endif
   if (tid == 0) {
     for (int i = 0; i < P8_RING; ++i) {
-      if (rank == 0) p8_mbar_init(&sh.empty[i], 1);
-      else p8_mbar_init(&sh.full[i], P8_WARPS);
+      if (rank == 0) mbar_init(&sh.empty[i], 1);
+      else mbar_init(&sh.full[i], P8_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }

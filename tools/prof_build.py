@@ -56,6 +56,16 @@ P8_CLASSES = ["byte boundary", "inside a byte", "same bucket", "same bucket, cla
 
 P8_PROF_N = P8_SLOTS - 1   # the model CTA's bits in a row
 
+# FXCM's slots. 0-6 add up to the model CTA's bit (12 and 13 split lane 0's share of slot 0; the rest of it is the
+# barrier), 16-20 to the mixer CTA's.
+FX_LABELS = {
+    0: "model CTA: bookkeeping", 1: "model CTA: unit offsets", 2: "model CTA: probe", 3: "model CTA: apply",
+    4: "model CTA: map epilogue, selectors", 5: "model CTA: waiting for a free ring slot", 6: "model CTA: handing the bit over",
+    12: "  of 0, lane 0: bit_head_model", 13: "  of 0, lane 0: text_byte at the byte boundary",
+    16: "mixer CTA: error terms, failure history", 17: "mixer CTA: SGD", 18: "mixer CTA: waiting for the model CTA",
+    19: "mixer CTA: row moves, dot products", 20: "mixer CTA: squash, final mixers, APMs",
+}
+
 
 def paq8_classes(a):
     """The model CTA's cycles per bit by phase and unit, one column per class of bit (row 1 = rows 2-5)."""
@@ -124,10 +134,10 @@ def run(n_bytes):
         print("%s: cycles per bit by phase (byte-boundary bits | other bits); clock %.0f MHz" % (name, sm_mhz))
         for k in range(a.shape[1]):
             if a[0, k] or a[1, k]:
-                print("  phase %2d  %9.0f | %9.0f   %s" % (k, a[0, k] / n_bytes, a[1, k] / (7 * n_bytes), P8_LABELS.get(k, "") if name == "paq8" else ""))
-        # PAQ8 runs on two CTAs: the model CTA counts in slots 0-15 (10: waiting for a free ring slot), the mixer CTA in
-        # 16-23 (16: waiting for a full slot); each CTA's total is its time per bit, less the mixer CTA's code-row writes
-        parts = (("model CTA", 0, 16), ("mixer CTA", 16, 24)) if name == "paq8" else (("total", 0, 24),)
+                print("  phase %2d  %9.0f | %9.0f   %s" % (k, a[0, k] / n_bytes, a[1, k] / (7 * n_bytes), (P8_LABELS if name == "paq8" else FX_LABELS).get(k, "")))
+        # PAQ8 and FXCM run on two CTAs: PAQ8's model CTA counts in slots 0-15 (10: waiting for a free ring slot), FXCM's in
+        # 0-11, their mixer CTAs in 16-23; each CTA's total is its time per bit, less the mixer CTA's code-row writes
+        parts = (("model CTA", 0, 16), ("mixer CTA", 16, 24)) if name == "paq8" else (("model CTA", 0, 12), ("mixer CTA", 16, 24))
         for label, lo, hi in parts:
             print("  %-9s %9.0f | %9.0f   -> %.1f us/bit average" % (label, a[0, lo:hi].sum() / n_bytes, a[1, lo:hi].sum() / (7 * n_bytes),
                                                                     a[:, lo:hi].sum() / (8 * n_bytes) / sm_mhz))
