@@ -4,8 +4,10 @@
 //  * every context of every context map is a lane (210 lanes for the sixteen 7-slot maps on warps 0-6, 63 for the three
 //    history maps on warps 7-8): bucket probe, bit-history step, state maps and the 5 / 7 mixer inputs of a context are
 //    independent of the other contexts of its map as long as they touch different 64-byte buckets this bit. That is CHECKED
-//    per bit (touched_buckets, including the buckets a deferred history write-back will reach); a map with a clash is
-//    evaluated by one lane in the reference's order instead.
+//    per bit (touched_buckets, including the buckets a deferred history write-back will reach; on the staying bits of the
+//    7-slot maps, bpos 1, 3, 4, 6, 7, the slots a context reads and writes, cm_slot_keys); a map with a clash is evaluated
+//    by one lane in the reference's order instead. On a staying bit a 7-slot lane reads its slot and run record from a
+//    copy in shared memory (P8CmCache).
 //  * the one global coupling of the 7-slot maps, the shared pseudo-random sequence that ages high-count states
 //    (paq8.cpp:1075), is resolved between the two passes: the draws themselves depend on the generator only, so one warp
 //    computes as many as a bit can take during the bookkeeping, 24 at a time (the generator is a lagged XOR:
@@ -60,7 +62,8 @@ enum { P8_SEEN = 4096, P8_RING = 4 };
 // P8_PROF_N counts the model CTA's bits of a row. 88+: the legs of a 7-slot map context's bit (P8_LEG: the longest lane of the
 // bit, each leg apart; not lane 0 on a bit with a clash, which walks the maps): probe 88 the state read, 89 touched_buckets,
 // 90 p8_claim; apply 91 the draw, 92 the store and the move to the next cell (bucket_find at bpos 2, 5, 0), 93 the run
-// record's input, 94 the cell's state and its StateMap load, 95 the other exports.
+// record's input, 94 the cell's state and its StateMap load, 95 the other exports. On a staying bit leg 88 includes the
+// start of both StateMap loads and 94 also counts the probe's wait for them after p8_claim.
 #ifdef P8_PROF
 enum { P8_PROF_ROWS = 6, P8_PROF_SLOTS = 128, P8_PROF_UNIT = 64, P8_PROF_LEG = 88, P8_PROF_N = P8_PROF_SLOTS - 1 };
 __device__ unsigned long long g_p8_prof[P8_PROF_ROWS][P8_PROF_SLOTS];
@@ -112,6 +115,16 @@ struct P8Slot {
   u8 c1, st_match_expected, st_text_first, st_text_mask;
 };
 
+// Each 7-slot map lane's copy of the 7 state bytes of its slot (t[cp0 ..]) and the 2 bytes of its run record (t[runp ..]):
+// a staying bit (cm_staying) reads only these, so its probe and apply take them from shared memory. Stores go through to
+// HBM, which stays the authority. A copy is filled where the lane's bucket line is read anyway: after the lane's apply on a
+// move bit (bpos 0, 2, 5), or at the probe of a staying bit while it is invalid. It is valid from the fill until the map
+// walks serially (p8_number) or the launch ends: contexts without a clash never write another's slot or run record.
+struct P8CmCache {
+  unsigned short sm[P8_CM_LANES][2];    // staying bit: smt[sm_cxt] and smt[the new cell's state], loaded by the probe
+  unsigned char slot[P8_CM_LANES][8], run[P8_CM_LANES][2], valid[P8_CM_LANES];
+};
+
 struct P8Shared {
   p8::State S;
   alignas(16) unsigned char tab[p8::TABLES_HOT_BYTES];
@@ -138,6 +151,7 @@ struct P8Shared {
     struct {                                                    // the model CTA
       unsigned long long seen[P8_SEEN];   // open-addressing set of (map, bucket) pairs touched this bit
       struct { double ch[3][32 * 33]; double pb[3][32]; } ols;   // Cholesky factor rows (padded) and a product buffer; byte boundaries only
+      P8CmCache cc;
 #ifdef P8_PROF
       long long leg_t[P8_CM_LANES];      // P8_LEG: when a lane's current leg started
 #endif
@@ -353,7 +367,38 @@ __device__ __noinline__ void p8_probe_cm2(P8Shared& sh, int tid, int bpos, int m
   const int n = i < m.index ? p8::cm2_touched(m, i, bpos, ids) : 0;
   if (n && p8_claim(sh.u.md.seen, P8_N_CM + k, ids, n)) sh.clash2[k] = 1;
 }
-// pass 1 of the 7-slot maps (warps 0-6, whole warps): aged state, draw flag, touched buckets
+// copy context i's slot and run record from HBM into lane tid's P8CmCache entry
+__device__ __forceinline__ void p8_cm_fill(P8CmCache& cc, const p8::Cm& m, int i, int tid) {
+  const unsigned char* s = m.t + m.cp0[i];
+  unsigned char v[9];          // every load before the first store: one round trip, not one per byte
+#pragma unroll
+  for (int j = 0; j < 7; ++j) v[j] = s[j];
+  v[7] = m.t[m.runp[i]];
+  v[8] = m.t[m.runp[i] + 1];
+#pragma unroll
+  for (int j = 0; j < 7; ++j) cc.slot[tid][j] = v[j];
+  cc.run[tid][0] = v[7];
+  cc.run[tid][1] = v[8];
+  cc.valid[tid] = 1;
+}
+// cm_step on a staying bit from lane tid's copy (P8CmCache) and the StateMap cells its probe loaded
+__device__ __forceinline__ int p8_cm_stay(P8CmCache& cc, p8::Cm& m, int i, int tid, p8::Out& o, int ns, int y, int c0, int bp) {
+  using namespace p8;
+  const p8::Tables& T = *o.T;
+  u8* sl = cc.slot[tid];
+  const int base = m.cp0[i];
+  if (m.cp[i] != P8_NULL) { m.t[m.cp[i]] = (u8)ns; sl[m.cp[i] - base] = (u8)ns; }
+  const int nc = cm_stay_cell(cc.run[tid][0], c0, bp);
+  m.cp[i] = nc >= 0 ? base + nc : P8_NULL;
+  if ((bp == 1 || bp == 4) && nc >= 0) bucket_prefetch2(m.t, m.mask, m.cxt[i], (u32)c0 * 2);
+  P8_LEG(4);
+  cm_run_input(T, o, cc.run[tid][0], cc.run[tid][1], c0, bp);
+  P8_LEG(5);
+  const int s = nc >= 0 ? sl[nc] : 0, so = m.sm_cxt[i];
+  m.sm_cxt[i] = s;
+  return cm_cell_inputs(T, o, m.sm_t + i * 256, so, cc.sm[tid][0], s, cc.sm[tid][1], y);
+}
+// pass 1 of the 7-slot maps (warps 0-6, whole warps): aged state, draw flag, touched buckets (slots on a staying bit)
 __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, int bpos) {
   using namespace p8;
   int k, i;
@@ -363,12 +408,24 @@ __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, i
     int ns = -1;
     if (i < m.cn) {
       P8_LEG(-1);
-      ns = cm_next_state(*sh.S.T, m, i, y);
+      const bool stay = cm_staying(bpos);
+      P8CmCache& cc = sh.u.md.cc;
+      u16 sm_old = 0, sm_new = 0;
+      if (stay) {         // the new cell is known before the bit's stores (c0 holds y), so both StateMap loads start here
+        if (!cc.valid[tid]) p8_cm_fill(cc, m, i, tid);
+        const u8* sl = cc.slot[tid];
+        ns = m.cp[i] != P8_NULL ? sh.S.T->state[sl[m.cp[i] - m.cp0[i]]][y] : -1;
+        const int nc = cm_stay_cell(cc.run[tid][0], c0, bpos);
+        const u16* smt = m.sm_t + i * 256;
+        sm_old = smt[m.sm_cxt[i]];
+        sm_new = smt[nc >= 0 ? sl[nc] : 0];
+      } else ns = cm_next_state(*sh.S.T, m, i, y);
       P8_LEG(0);
-      const int n = cm_touched(m, i, c0, bpos, sh.ids[tid]);
+      const int n = stay ? cm_slot_keys(m, i, sh.ids[tid]) : cm_touched(m, i, c0, bpos, sh.ids[tid]);
       P8_LEG(1);
       if (p8_claim(sh.u.md.seen, k, sh.ids[tid], n)) { sh.clash[k] = 1; sh.any_clash = 1; }
       P8_LEG(2);
+      if (stay) { cc.sm[tid][0] = sm_old; cc.sm[tid][1] = sm_new; P8_LEG(6); }
     }
     sh.ns[tid] = (short)ns;
     flag = ns >= 204;
@@ -459,6 +516,8 @@ __device__ __noinline__ void p8_apply_cm(P8Shared& sh, int tid, int y, int c0, i
   int k, i;
   if (!p8_cm_lane(tid, k, i)) return;
   Cm& m = p8_cm(sh.S, k);
+  P8CmCache& cc = sh.u.md.cc;
+  if (sh.clash[k]) cc.valid[tid] = 0;      // lane 0 walks the map serially
   if (sh.clash[k] || i >= m.cn) return;
   P8_LEG(-1);
   int ns = sh.ns[tid];
@@ -468,7 +527,11 @@ __device__ __noinline__ void p8_apply_cm(P8Shared& sh, int tid, int y, int c0, i
   }
   P8_LEG(3);
   Out o = p8_out(sh, sh.unit_off[c_p8_cm_unit[k]] + 5 * i);
-  cm_step(m, i, o, ns, y, c0, bpos, buf(sh.S, 1));
+  if (cm_staying(bpos)) p8_cm_stay(cc, m, i, tid, o, ns, y, c0, bpos);
+  else {
+    cm_step(m, i, o, ns, y, c0, bpos, buf(sh.S, 1));
+    p8_cm_fill(cc, m, i, tid);
+  }
 }
 // DMC forest combination, and the reset at a byte boundary (dmcForest::mix), from the dmc_st values of the probe
 __device__ __forceinline__ void p8_dmc_mix(P8Shared& sh, p8::Out& o, int bpos) {
@@ -1049,6 +1112,7 @@ __device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g
   const p8::Tables* gT = sh.S.T;
   p8_copy_words(sh.tab, gT, p8::TABLES_HOT_BYTES, tid);
   if (tid < p8::N_SETS) sh.wc_set[tid] = -1;
+  if (rank == 0) for (int k = tid; k < P8_CM_LANES; k += P8_THREADS) sh.u.md.cc.valid[k] = 0;   // shared memory is new
 #ifdef P8_PROF
   for (int k = tid; k < P8_PROF_SLOTS; k += P8_THREADS) sh.prof_acc[k] = 0;
 #endif

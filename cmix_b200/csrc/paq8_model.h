@@ -33,6 +33,11 @@
 #ifndef P8_CENSUS_CM2
 #define P8_CENSUS_CM2(m, bpos) do { } while (0)
 #endif
+// Host test of the clash rule (tools/census.h with -DCENSUS_REVERSE): may evaluate cm_mix's contexts in another order and
+// return. Empty in every product build.
+#ifndef P8_CM_ORDER
+#define P8_CM_ORDER(T, m, o, rnd, y, c0, bp, c1) do { } while (0)
+#endif
 // Profiling build of the device (paq8.cuh with -DP8_PROF): the end of leg k of a 7-slot map context's bit. Empty elsewhere.
 #ifndef P8_LEG
 #define P8_LEG(k) do { } while (0)
@@ -338,6 +343,46 @@ P8_HD inline int touched_buckets(const u8* t, u32 mask, int cell, int run, u32 c
   return n;
 }
 P8_HD inline int cm_touched(const Cm& m, int i, int c0, int bp, u32* ids) { return touched_buckets(m.t, m.mask, m.cp[i], m.runp[i], m.cxt[i], m.chk[i], (u32)c0, bp, ids); }
+// A staying bit (bp 1, 3, 4, 6, 7) keeps every context of a 7-slot map in its slot: cm_step neither calls bucket_find nor
+// updates a run record. Context i then writes only t[cp], in its current slot, and reads only that slot and t[runp], t[runp+1]
+// (its StateMap row is its own), so contexts whose slots differ commute. Its keys: the base offsets of its current slot (none
+// when the cell is null) and of its run record's slot. Other bits touch whole buckets (cm_touched).
+P8_HD inline bool cm_staying(int bp) { return (0xDA >> bp) & 1; }
+P8_HD inline int cm_slot_keys(const Cm& m, int i, u32* ids) {
+  int n = 0;
+  if (m.cp[i] != P8_NULL) ids[n++] = (u32)m.cp0[i];
+  ids[n++] = (u32)(m.runp[i] - 3);
+  return n;
+}
+// The input of a context's run record (r0, r1: its count and byte).
+P8_HD inline void cm_run_input(const Tables& T, Out& o, int r0, int r1, int c0, int bp) {
+  if (((r1 + 256) >> (8 - bp)) == c0) {
+    const int b = ((r1 >> (7 - bp)) & 1) * 2 - 1;
+    const int c = ilog(T, r0 + 1) << (2 + (~r0 & 1));
+    add(o, b * c);
+  } else add(o, 0);
+}
+// The StateMap16 update of the previous bit's cell `so` (sm_old = smt[so]) and the four inputs of the new cell's state s
+// (fresh = smt[s], both read before the update is stored).
+P8_HD inline int cm_cell_inputs(const Tables& T, Out& o, u16* smt, int so, u16 sm_old, int s, u16 fresh, int y) {
+  const u16 upd = (u16)(sm_old + (((y << 16) - (int)sm_old + 128) >> 8));
+  if (s == so) fresh = upd;
+  smt[so] = upd;
+  const int p1 = fresh >> 4;
+  const int st = (stretch(T, p1) + 2) >> 2;
+  add(o, st); P8_LEG(6);
+  add(o, (p1 - 2047 + 4) >> 3);
+  const int n0 = -!T.state[s][2], n1 = -!T.state[s][3];
+  add(o, st * iabs(n1 - n0));
+  const int p0 = 4095 - p1;
+  add(o, ((p1 & n0) - (p0 & n1) + 8) >> 4); P8_LEG(7);
+  return s > 0;
+}
+// The cell a context moves to on a staying bit, as its index in the slot (-1: null), from its run record's count r0.
+P8_HD inline int cm_stay_cell(int r0, int c0, int bp) {
+  if (bp > 1 && r0 == 0) return -1;
+  return (bp == 4 || bp == 7) ? 3 + (c0 & 3) : 1 + (c0 & 1);
+}
 // One context of one bit: store the aged state `ns` (already decided, -1 = no cell), move to the next cell, emit 5 inputs at o.
 P8_HD inline int cm_step(Cm& m, int i, Out& o, int ns, int y, int c0, int bp, int c1) {
   const Tables& T = *o.T;
@@ -366,32 +411,16 @@ P8_HD inline int cm_step(Cm& m, int i, Out& o, int ns, int y, int c0, int bp, in
   }
   if ((bp == 1 || bp == 4) && m.cp[i] != P8_NULL) bucket_prefetch2(t, m.mask, m.cxt[i], (u32)c0 * 2); P8_LEG(4);
   const u8* rp = t + m.runp[i];
-  const int rc = rp[0];
-  if (((rp[1] + 256) >> (8 - bp)) == c0) {
-    const int b = ((rp[1] >> (7 - bp)) & 1) * 2 - 1;
-    const int c = ilog(T, rc + 1) << (2 + (~rc & 1));
-    add(o, b * c);
-  } else add(o, 0);
+  cm_run_input(T, o, rp[0], rp[1], c0, bp);
   P8_LEG(5); const int s = m.cp[i] != P8_NULL ? t[m.cp[i]] : 0;
-  u16 fresh = smt[s];
-  const u16 upd = (u16)(sm_old + (((y << 16) - (int)sm_old + 128) >> 8));   // StateMap16 update of the previous bit's cell
-  if (s == so) fresh = upd;
-  smt[so] = upd;
   m.sm_cxt[i] = s;
-  const int p1 = fresh >> 4;
-  const int st = (stretch(T, p1) + 2) >> 2;
-  add(o, st); P8_LEG(6);
-  add(o, (p1 - 2047 + 4) >> 3);
-  const int n0 = -!T.state[s][2], n1 = -!T.state[s][3];
-  add(o, st * iabs(n1 - n0));
-  const int p0 = 4095 - p1;
-  add(o, ((p1 & n0) - (p0 & n1) + 8) >> 4); P8_LEG(7);
-  return s > 0;
+  return cm_cell_inputs(T, o, smt, so, sm_old, s, smt[s], y);
 }
 // The in-order loop. `rnd` is the global generator: draws happen in context order.
 P8_COLD P8_HD inline int cm_mix(Cm& m, Out& o, Rnd& rnd, int y, int c0, int bp, int c1) {
   const Tables& T = *o.T;
   P8_CENSUS_CM(T, m, y, c0, bp);
+  P8_CM_ORDER(T, m, o, rnd, y, c0, bp, c1);
   int result = 0;
   for (int i = 0; i < m.cn; ++i) {
     int ns = cm_next_state(T, m, i, y);
