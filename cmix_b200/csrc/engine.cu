@@ -29,6 +29,7 @@
 #include "../../include/cmixb200.h"
 #include "exact_math.h"
 #include "jitter.cuh"
+#include "census.cuh"
 #include "coder.cuh"
 #include "fxcm_model.h"
 #include "fxcm_host.h"
@@ -931,10 +932,16 @@ int cmixb200_create_ex(const uint8_t vocab[256], const char* dictionary_path, in
   return CMIXB200_OK;
 }
 
+#ifdef CMIXB200_CENSUS
+int cmixb200_census_detach(cmixb200_predictor* P);
+#endif
 void cmixb200_destroy(cmixb200_predictor* P) {
   if (!P) return;
   cudaSetDevice(P->device);
   cudaDeviceSynchronize();
+#ifdef CMIXB200_CENSUS
+  cmixb200_census_detach(P);           // its memory may be a later predictor's
+#endif
   for (void* q : P->allocs) cudaFree(q);
   for (cudaEvent_t e : {P->ev_lock_mix, P->ev_lock_small, P->ev_lock_p8}) if (e) cudaEventDestroy(e);
   for (int i = 0; i < 8; ++i) if (P->ev[i]) cudaEventDestroy(P->ev[i]);
@@ -1342,6 +1349,82 @@ extern "C" int cmixb200_jitter_counts(unsigned* out, size_t n) {
     const cudaError_t e = get(out);
     if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return CMIXB200_ERR_CUDA; }
   }
+  return CMIXB200_OK;
+}
+#endif
+
+#ifdef CMIXB200_CENSUS
+// Census build only (census.cuh): a per-bit log of the clash verdicts of PAQ8 and FXCM and of PAQ8's slot-cache checks per
+// predictor. Not in include/cmixb200.h: a product build does not have them.
+namespace cmixb200 {
+static CensusEntry g_census[CENSUS_STREAMS];
+static cmixb200_predictor* g_census_owner[CENSUS_STREAMS];
+static int census_upload() {
+  for (auto set : {census_set_paq8, census_set_fxcm}) CK(set(g_census));
+  return CMIXB200_OK;
+}
+static int census_slot(cmixb200_predictor* P) {
+  for (int k = 0; k < CENSUS_STREAMS; ++k) if (g_census_owner[k] == P) return k;
+  return -1;
+}
+}  // namespace cmixb200
+extern "C" int cmixb200_census_detach(cmixb200_predictor* P) {
+  const int k = census_slot(P);
+  if (k < 0) return CMIXB200_OK;
+  CK(cudaSetDevice(P->device));
+  CK(cudaDeviceSynchronize());
+  for (void* q : {(void*)g_census[k].head, (void*)g_census[k].p8, (void*)g_census[k].fx}) cudaFree(q);
+  g_census[k] = CensusEntry{};
+  g_census_owner[k] = nullptr;
+  return census_upload();
+}
+// Logs up to cap_bits bits of P's PAQ8 and FXCM from the next launch on (a predictor already attached starts afresh).
+extern "C" int cmixb200_census_attach(cmixb200_predictor* P, unsigned cap_bits) {
+  TRY(cmixb200_census_detach(P));
+  int k = census_slot(nullptr);
+  if (k < 0) { g_last_error = "census: every log is attached"; return CMIXB200_ERR_ARG; }
+  CK(cudaSetDevice(P->device));
+  CensusEntry e{};
+  if (P->d_p8) CK(cudaMemcpy(&e.p8_key, (const char*)P->d_p8 + offsetof(p8::State, sparse.cm.t), sizeof(void*), cudaMemcpyDeviceToHost));
+  if (P->d_fx) CK(cudaMemcpy(&e.fx_key, (const char*)P->d_fx + offsetof(fx::State, map[0].t), sizeof(void*), cudaMemcpyDeviceToHost));
+  CK(cudaMalloc(&e.head, sizeof(CensusHead)));
+  CK(cudaMalloc(&e.p8, (size_t)cap_bits * CENSUS_P8_WORDS * 4 + 4));
+  CK(cudaMalloc(&e.fx, (size_t)cap_bits * 4 + 4));
+  CensusHead h{};
+  h.cap = cap_bits;
+  CK(cudaMemcpy(e.head, &h, sizeof h, cudaMemcpyHostToDevice));
+  g_census[k] = e;
+  g_census_owner[k] = P;
+  return census_upload();
+}
+// head: the 16 words of CensusHead; p8 / fx: the first n_bits records (3 / 1 u32 each; either may be null)
+extern "C" int cmixb200_census_read(cmixb200_predictor* P, unsigned* head, unsigned* p8, unsigned* fx, size_t n_bits) {
+  const int k = census_slot(P);
+  if (k < 0) { g_last_error = "census: no log attached"; return CMIXB200_ERR_ARG; }
+  CK(cudaSetDevice(P->device));
+  CK(cudaDeviceSynchronize());
+  CensusHead h;
+  CK(cudaMemcpy(&h, g_census[k].head, sizeof h, cudaMemcpyDeviceToHost));
+  if (n_bits > h.cap) { g_last_error = "census: more bits than the log holds"; return CMIXB200_ERR_ARG; }
+  memcpy(head, &h, sizeof h);
+  if (p8 && n_bits) CK(cudaMemcpy(p8, g_census[k].p8, n_bits * CENSUS_P8_WORDS * 4, cudaMemcpyDeviceToHost));
+  if (fx && n_bits) CK(cudaMemcpy(fx, g_census[k].fx, n_bits * 4, cudaMemcpyDeviceToHost));
+  return CMIXB200_OK;
+}
+// Empties P's log and its counters.
+extern "C" int cmixb200_census_reset(cmixb200_predictor* P) {
+  const int k = census_slot(P);
+  if (k < 0) { g_last_error = "census: no log attached"; return CMIXB200_ERR_ARG; }
+  CK(cudaSetDevice(P->device));
+  CK(cudaDeviceSynchronize());
+  CensusHead h;
+  CK(cudaMemcpy(&h, g_census[k].head, sizeof h, cudaMemcpyDeviceToHost));
+  const unsigned cap = h.cap;
+  h = CensusHead{};
+  h.cap = cap;
+  CK(cudaMemcpy(g_census[k].head, &h, sizeof h, cudaMemcpyHostToDevice));
+  CK(cudaMemset(g_census[k].p8, 0, (size_t)cap * CENSUS_P8_WORDS * 4));
+  CK(cudaMemset(g_census[k].fx, 0, (size_t)cap * 4));
   return CMIXB200_OK;
 }
 #endif

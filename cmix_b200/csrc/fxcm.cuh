@@ -27,6 +27,7 @@
 #include "fxcm_model.h"
 #include "bytemodel.cuh"
 #include "state.h"
+#include "census.cuh"
 
 namespace cmixb200 {
 
@@ -233,6 +234,7 @@ __device__ void fx_model_bit(FxShared& sh, FxSlot* ring, u32 t, int y, int lstmp
     if (u >= 0) bit_unit(S, u);
   }
   JIT_SYNCTHREADS();
+  if (tid == 0) CENSUS_FX_BIT(S.map[0].t, sh.u.md.clash);   // the bit's verdicts are final here
   FX_T(2);
   // ---- D: the map contexts
   if (tid < FX_MAP_LANES) {

@@ -19,6 +19,9 @@ void fxcm_launch_bit(StreamState* st, fx::State* g, int y, int pretrain, u16* ex
 #ifdef CMIXB200_JITTER
 JIT_MODULE(fxcm)
 #endif
+#ifdef CMIXB200_CENSUS
+CENSUS_MODULE(fxcm)
+#endif
 
 }  // namespace cmixb200
 

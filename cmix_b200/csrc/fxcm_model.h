@@ -30,6 +30,11 @@
 #ifndef FX_CENSUS_MAP
 #define FX_CENSUS_MAP(S, id) do { } while (0)
 #endif
+// Host test of the clash rule (tools/census.h with -DCENSUS_PERMUTE): may evaluate map_bit's contexts in another order and
+// return. Empty in every product build.
+#ifndef FX_MAP_ORDER
+#define FX_MAP_ORDER(S, id, o) do { } while (0)
+#endif
 
 namespace cmixb200 {
 namespace fx {
@@ -337,6 +342,7 @@ FX_HD inline void map_finish(State& S, int id, u32 result) {
 // One bit of one context map, contexts in order (mix / mix1).
 FX_HD inline void map_bit(State& S, int id, Out& o) {
   FX_CENSUS_MAP(S, id);
+  FX_MAP_ORDER(S, id, o);
   u32 result = 0;
   const int cn = S.map[id].cn;
   for (int i = 0; i < cn; ++i) result += map_ctx_bit(S, id, i, o);

@@ -46,6 +46,7 @@ namespace cmixb200 { __host__ __device__ inline void p8_leg(int k); }
 #endif
 #include "paq8_top.h"
 #include "state.h"
+#include "census.cuh"
 
 namespace cmixb200 {
 
@@ -381,12 +382,14 @@ __device__ __forceinline__ void p8_cm_fill(P8CmCache& cc, const p8::Cm& m, int i
   cc.run[tid][1] = v[8];
   cc.valid[tid] = 1;
 }
-// cm_step on a staying bit from lane tid's copy (P8CmCache) and the StateMap cells its probe loaded
-__device__ __forceinline__ int p8_cm_stay(P8CmCache& cc, p8::Cm& m, int i, int tid, p8::Out& o, int ns, int y, int c0, int bp) {
+// cm_step on a staying bit from lane tid's copy (P8CmCache) and the StateMap cells its probe loaded (k: the map's index,
+// key: the stream's, for the census build)
+__device__ __forceinline__ int p8_cm_stay(P8CmCache& cc, p8::Cm& m, int i, int tid, p8::Out& o, int ns, int y, int c0, int bp, int k, const void* key) {
   using namespace p8;
   const p8::Tables& T = *o.T;
   u8* sl = cc.slot[tid];
   const int base = m.cp0[i];
+  CENSUS_P8_COPY(key, m, k, i, sl, cc.run[tid], false, false);
   if (m.cp[i] != P8_NULL) { m.t[m.cp[i]] = (u8)ns; sl[m.cp[i] - base] = (u8)ns; }
   const int nc = cm_stay_cell(cc.run[tid][0], c0, bp);
   m.cp[i] = nc >= 0 ? base + nc : P8_NULL;
@@ -396,6 +399,7 @@ __device__ __forceinline__ int p8_cm_stay(P8CmCache& cc, p8::Cm& m, int i, int t
   P8_LEG(5);
   const int s = nc >= 0 ? sl[nc] : 0, so = m.sm_cxt[i];
   m.sm_cxt[i] = s;
+  CENSUS_P8_SM(key, k, i, m.sm_t + i * 256, so, cc.sm[tid][0], s, cc.sm[tid][1]);
   return cm_cell_inputs(T, o, m.sm_t + i * 256, so, cc.sm[tid][0], s, cc.sm[tid][1], y);
 }
 // pass 1 of the 7-slot maps (warps 0-6, whole warps): aged state, draw flag, touched buckets (slots on a staying bit)
@@ -412,7 +416,11 @@ __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, i
       P8CmCache& cc = sh.u.md.cc;
       u16 sm_old = 0, sm_new = 0;
       if (stay) {         // the new cell is known before the bit's stores (c0 holds y), so both StateMap loads start here
+#ifdef CMIXB200_CENSUS
+        const bool filled = !cc.valid[tid];
+#endif
         if (!cc.valid[tid]) p8_cm_fill(cc, m, i, tid);
+        CENSUS_P8_COPY(sh.S.sparse.cm.t, m, k, i, cc.slot[tid], cc.run[tid], true, filled);
         const u8* sl = cc.slot[tid];
         ns = m.cp[i] != P8_NULL ? sh.S.T->state[sl[m.cp[i] - m.cp0[i]]][y] : -1;
         const int nc = cm_stay_cell(cc.run[tid][0], c0, bpos);
@@ -527,7 +535,7 @@ __device__ __noinline__ void p8_apply_cm(P8Shared& sh, int tid, int y, int c0, i
   }
   P8_LEG(3);
   Out o = p8_out(sh, sh.unit_off[c_p8_cm_unit[k]] + 5 * i);
-  if (cm_staying(bpos)) p8_cm_stay(cc, m, i, tid, o, ns, y, c0, bpos);
+  if (cm_staying(bpos)) p8_cm_stay(cc, m, i, tid, o, ns, y, c0, bpos, k, sh.S.sparse.cm.t);
   else {
     cm_step(m, i, o, ns, y, c0, bpos, buf(sh.S, 1));
     p8_cm_fill(cc, m, i, tid);
@@ -970,6 +978,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       m.n2 = m.nx;
       while (m.nx & 7) m.tx[m.nx++] = 0;
       P8_U(23);
+      CENSUS_P8_BIT(S.sparse.cm.t, sh.clash, sh.clash2, sh.flag_mask, P8_CM_LANES, bpos);   // the bit's verdicts are final here
 #ifdef P8_PROF
       prof_clash = sh.any_clash != 0;
 #endif

@@ -19,6 +19,9 @@ void paq8_launch_bit(p8::State* g, int y, u16* ext_bit, cudaStream_t s, const u3
 #ifdef CMIXB200_JITTER
 JIT_MODULE(paq8)
 #endif
+#ifdef CMIXB200_CENSUS
+CENSUS_MODULE(paq8)
+#endif
 
 }  // namespace cmixb200
 

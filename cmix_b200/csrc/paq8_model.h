@@ -33,10 +33,13 @@
 #ifndef P8_CENSUS_CM2
 #define P8_CENSUS_CM2(m, bpos) do { } while (0)
 #endif
-// Host test of the clash rule (tools/census.h with -DCENSUS_REVERSE): may evaluate cm_mix's contexts in another order and
-// return. Empty in every product build.
+// Host test of the clash rule (tools/census.h with -DCENSUS_PERMUTE / -DCENSUS_REVERSE): may evaluate cm_mix's /
+// cm2_mix_body's contexts in another order and return. Empty in every product build.
 #ifndef P8_CM_ORDER
 #define P8_CM_ORDER(T, m, o, rnd, y, c0, bp, c1) do { } while (0)
+#endif
+#ifndef P8_CM2_ORDER
+#define P8_CM2_ORDER(m, o, y, bpos) do { } while (0)
 #endif
 // Profiling build of the device (paq8.cuh with -DP8_PROF): the end of leg k of a 7-slot map context's bit. Empty elsewhere.
 #ifndef P8_LEG
@@ -538,6 +541,7 @@ P8_HD inline int cm2_step(Cm2& m, int i, Out& o, int y, int bpos) {
 // In-order evaluation. The reference updates ALL contexts before predicting from any (two loops); the per-context fusion
 // below is the same computation whenever the contexts touch disjoint buckets this bit, and the two-loop order otherwise.
 P8_COLD P8_HD inline int cm2_mix_body(Cm2& m, Out& o, int y, int bpos) {   // after cm2_begin(), before the byte-end reset of `index`
+  P8_CM2_ORDER(m, o, y, bpos);
   const Tables& T = *o.T;
   u8* t = m.t;
   // loop 1 (Update): cells and pointers only

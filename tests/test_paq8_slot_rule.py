@@ -6,7 +6,9 @@ clashes walks serially (p8_number / cm_mix). CPU only:
   * the census (tools/census.h, the device's rule on the host) finds no staying-bit clash in full_text / full_bin, while the
     stress fixtures still reach the serial walk on such a bit;
   * a host build that evaluates the contexts of every clash-free map of a staying bit in REVERSE order (each flagged
-    context taking the draw of its in-order rank, as the device's lanes do) reproduces the reference's PAQ8 codes."""
+    context taking the draw of its in-order rank, as the device's lanes do) reproduces the reference's PAQ8 codes.
+tests/test_device_census.py generalises the second test to a seeded random order on every bit, in the history maps and
+FXCM's maps too (-DCENSUS_PERMUTE), and pins the device's per-bit verdicts to this census."""
 import os
 from concurrent.futures import ThreadPoolExecutor
 

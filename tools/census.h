@@ -13,6 +13,20 @@
 //   draw_bits, max_draws             bits with any draw of the shared sequence, the most draws in one bit
 //   gt24, gt24_fast                  bits with more than 24 draws; of those, bits without a 7-slot clash (the replay path)
 // Include it before paq8_host.h / fxcm_host.h; call end_bit() after every bit and reset() after pretraining.
+//
+// Per-bit log (open_log; the census build of the device library writes the same words, paq8.cuh / fxcm.cuh CENSUS_*):
+//   PAQ8, 3 u32 per bit   w0 = clashing 7-slot maps (bit k: map k of p8_cm's order) | clashing history maps << 16 | bpos << 20
+//                         w1 = flagged draws | copies of P8CmCache the probe checks << 16 (the cn of every 7-slot map on a
+//                              staying bit, 0 on a move bit)
+//                         w2 = the 7-slot maps that clash under the bucket rule (cm_touched on every bit)
+//   FXCM, 1 u32 per bit   the clashing maps among the 31
+// The device's third PAQ8 word is not w2 but the copies its probe filled (the host has no cache).
+//
+// -DCENSUS_PERMUTE=<seed>: in every map the rule finds clash-free, the contexts are evaluated in a seeded pseudo-random
+// order instead of in order, on every bit and in all three families (cm_mix: each flagged context takes the draw of its
+// in-order rank, as the device's lanes do; cm2_mix_body; fxcm_model.h map_bit). If the rule is right, the codes stay the
+// reference's. "permuted" in the JSON line counts the map-bits whose order changed. -DCENSUS_REVERSE: the reverse order, on
+// the 7-slot maps' staying bits only.
 #pragma once
 #include <stdint.h>
 #include <stdio.h>
@@ -28,13 +42,30 @@ namespace census {
 struct Counts {
   int draws = 0, bp = 0;                         // this bit
   bool clash7 = false, bucket7 = false, clash_hist = false, fx_clash = false;
+  uint32_t mask7 = 0, mask_bucket = 0, mask_hist = 0, mask_fx = 0, checked = 0;
   long bits = 0, draw_bits = 0, max_draws = 0, gt24 = 0, gt24_fast = 0, clash7_bits = 0, clash_hist_bits = 0, fx_clash_bits = 0;
-  long clash7_stay = 0, clash7_bpos[8] = {}, bucket7_bpos[8] = {};
+  long clash7_stay = 0, clash7_bpos[8] = {}, bucket7_bpos[8] = {}, permuted = 0;
   std::map<const void*, long> p8_map;            // PAQ8 map -> bits with a clash in it
   std::map<int, long> fx_map;                    // FXCM map id -> bits with a clash in it
 };
 inline Counts& C() { static Counts c; return c; }
+inline std::map<const void*, int>& order() { static std::map<const void*, int> o; return o; }   // PAQ8 map -> index (device order)
+struct Log { FILE* f = nullptr; bool fx = false; };
+inline Log& L() { static Log l; return l; }
 inline void reset() { C() = Counts(); }
+
+// The PAQ8 maps in the device's order: the sixteen 7-slot maps of p8_cm, then the three history maps of p8_cm2.
+inline void set_maps(const std::vector<std::pair<std::string, const void*>>& maps) {
+  for (size_t k = 0; k < maps.size(); ++k) order()[maps[k].second] = (int)k;
+}
+inline uint32_t map_flag(const void* m) {    // bit k: map k of set_maps' list
+  auto it = order().find(m);
+  return it == order().end() ? 0u : 1u << it->second;
+}
+// The per-bit log; path nullptr: none. fx: the FXCM layout.
+inline void open_log(const char* path, bool fx) {
+  if (path && *path) { L().f = fopen(path, "wb"); L().fx = fx; }
+}
 
 // p8_claim / fx_claim: a context's own repeats are removed; a bucket another context of the map touched this bit is a clash
 inline bool claim(std::set<uint32_t>& seen, const uint32_t* ids, int n) {
@@ -68,31 +99,91 @@ template <class Tab, class Map> void p8_cm(const Tab& T, const Map& m, int y, in
   }
   C().bp = bp;
   C().bucket7 |= bucket;
-  if (p8_cm_clash(m, c0, bp)) { C().clash7 = true; ++C().p8_map[&m]; }
+  if (bucket) C().mask_bucket |= map_flag(&m);
+  if (staying(bp)) C().checked += m.cn;
+  if (p8_cm_clash(m, c0, bp)) { C().clash7 = true; C().mask7 |= map_flag(&m); ++C().p8_map[&m]; }
 }
+
+#if defined(CENSUS_PERMUTE) || defined(CENSUS_REVERSE)
+// The order of n contexts: a seeded Fisher-Yates shuffle (one generator over the run), or the reverse order.
+inline void order_of(int n, int* perm) {
+  for (int i = 0; i < n; ++i) perm[i] = i;
+#ifdef CENSUS_PERMUTE
+  static uint64_t s = 0x9E3779B97F4A7C15ull ^ (uint64_t)(CENSUS_PERMUTE);
+  for (int i = n - 1; i > 0; --i) {
+    s ^= s << 13; s ^= s >> 7; s ^= s << 17;
+    const int j = (int)(s % (uint64_t)(i + 1));
+    const int t = perm[i]; perm[i] = perm[j]; perm[j] = t;
+  }
+#else
+  for (int i = 0; i < n; ++i) perm[i] = n - 1 - i;
+#endif
+  for (int i = 0; i < n; ++i) if (perm[i] != i) { ++C().permuted; break; }
+}
+// cm_mix on a map the rule finds clash-free: the contexts in order_of's order, each flagged context taking the draw of its
+// in-order rank (what the device's lanes do in any order) and storing the aged state pass 1 computed (p8_probe_cm).
+// Returns cm_mix's result, or -1 where cm_mix runs in order.
+template <class Tab, class Map, class Out, class Rnd> int p8_cm_order(const Tab& T, Map& m, Out& o, Rnd& rnd, int y, int c0, int bp, int c1) {
 #ifdef CENSUS_REVERSE
-// Test of the slot rule's exactness: on a staying bit where it finds no clash in map m, evaluate the contexts in REVERSE
-// order, each flagged context taking the draw of its in-order rank (what the device's lanes do in any order). Returns
-// cm_mix's result, or -1 where cm_mix runs in order.
-template <class Tab, class Map, class Out, class Rnd> int p8_cm_reverse(const Tab& T, Map& m, Out& o, Rnd& rnd, int y, int c0, int bp, int c1) {
-  if (!staying(bp) || p8_cm_clash(m, c0, bp)) return -1;
-  bool flag[64];
+  if (!staying(bp)) return -1;
+#endif
+  if (p8_cm_clash(m, c0, bp)) return -1;
+  int ns[64], perm[64];
   uint32_t draw[64];
   for (int i = 0; i < m.cn; ++i) {
-    flag[i] = cm_next_state(T, m, i, y) >= 204;
-    if (flag[i]) draw[i] = rnd_next(rnd);
+    ns[i] = cm_next_state(T, m, i, y);
+    if (ns[i] >= 204) draw[i] = rnd_next(rnd);
   }
+  order_of(m.cn, perm);
   int result = 0;
-  for (int i = m.cn - 1; i >= 0; --i) {
-    int ns = cm_next_state(T, m, i, y);
-    if (flag[i] && ns >= 204 && (uint32_t)(draw[i] << ((452 - ns) >> 3)) != 0) ns -= 4;   // cm_draw_hits
+  for (int q = 0; q < m.cn; ++q) {
+    const int i = perm[q];
+    int s = ns[i];
+    if (s >= 204 && (uint32_t)(draw[i] << ((452 - s) >> 3)) != 0) s -= 4;   // cm_draw_hits
     Out oi = o;
     oi.n = o.n + 5 * i;
-    result += cm_step(m, i, oi, ns, y, c0, bp, c1);
+    result += cm_step(m, i, oi, s, y, c0, bp, c1);
   }
   o.n += 5 * m.cn;
   if (bp == 7) m.cn = 0;
   return result;
+}
+#endif
+#ifdef CENSUS_PERMUTE
+// cm2_mix_body on a history map the rule finds clash-free: cm2_step per context (p8_apply_cm2's lanes) in order_of's order
+template <class Map, class Out> int p8_cm2_order(Map& m, Out& o, int y, int bpos) {
+  std::set<uint32_t> seen;
+  uint32_t ids[5];
+  for (int i = 0; i < m.index; ++i) {
+    const int n = cm2_touched(m, i, bpos, ids);
+    if (n && claim(seen, ids, n)) return -1;
+  }
+  int perm[64], result = 0;
+  order_of(m.index, perm);
+  for (int q = 0; q < m.index; ++q) {
+    Out oi = o;
+    oi.n = o.n + 7 * perm[q];
+    result += cm2_step(m, perm[q], oi, y, bpos);
+  }
+  o.n += 7 * m.index;
+  return result;
+}
+// map_bit on an FXCM map the rule finds clash-free: map_ctx_bit per context (fxcm.cuh phase D) in order_of's order.
+// Returns false where map_bit runs in order.
+template <class State, class Out> bool fx_map_order(State& S, int id, const Out& o) {
+  std::set<uint32_t> seen;
+  uint32_t ids[5];
+  const int cn = S.map[id].cn;
+  for (int i = 0; i < cn; ++i) {
+    const int n = map_touched(S, id, i, ids);
+    if (n && claim(seen, ids, n)) return false;
+  }
+  int perm[64];
+  uint32_t result = 0;
+  order_of(cn, perm);
+  for (int q = 0; q < cn; ++q) result += map_ctx_bit(S, id, perm[q], o);
+  map_finish(S, id, result);
+  return true;
 }
 #endif
 // p8_probe_cm2 (after cm2_begin)
@@ -104,7 +195,7 @@ template <class Map> void p8_cm2(const Map& m, int bpos) {
     const int n = cm2_touched(m, i, bpos, ids);
     if (n && claim(seen, ids, n)) clash = true;
   }
-  if (clash) { C().clash_hist = true; ++C().p8_map[&m]; }
+  if (clash) { C().clash_hist = true; C().mask_hist |= map_flag(&m) >> 16; ++C().p8_map[&m]; }
 }
 // fxcm.cuh phase C
 template <class State> void fx_map(const State& S, int id) {
@@ -115,11 +206,18 @@ template <class State> void fx_map(const State& S, int id) {
     const int n = map_touched(S, id, i, ids);
     if (n && claim(seen, ids, n)) clash = true;
   }
-  if (clash) { C().fx_clash = true; ++C().fx_map[id]; }
+  if (clash) { C().fx_clash = true; C().mask_fx |= 1u << id; ++C().fx_map[id]; }
 }
 
 inline void end_bit() {
   Counts& c = C();
+  if (L().f) {
+    if (L().fx) fwrite(&c.mask_fx, 4, 1, L().f);
+    else {
+      const uint32_t w[3] = {c.mask7 | c.mask_hist << 16 | (uint32_t)c.bp << 20, (uint32_t)c.draws | c.checked << 16, c.mask_bucket};
+      fwrite(w, 4, 3, L().f);
+    }
+  }
   ++c.bits;
   c.draw_bits += c.draws > 0;
   if (c.draws > c.max_draws) c.max_draws = c.draws;
@@ -133,14 +231,16 @@ inline void end_bit() {
   c.fx_clash_bits += c.fx_clash;
   c.draws = 0;
   c.clash7 = c.bucket7 = c.clash_hist = c.fx_clash = false;
+  c.mask7 = c.mask_bucket = c.mask_hist = c.mask_fx = c.checked = 0;
 }
 
 // One JSON line: "census {...}". `maps` names the PAQ8 maps (in the device's order); FXCM maps are named by id.
 inline void print(FILE* f, const std::vector<std::pair<std::string, const void*>>& maps) {
+  if (L().f) { fclose(L().f); L().f = nullptr; }
   const Counts& c = C();
   fprintf(f, "census {\"bits\": %ld, \"draw_bits\": %ld, \"max_draws\": %ld, \"gt24\": %ld, \"gt24_fast\": %ld, \"clash7\": %ld, "
-             "\"clash7_stay\": %ld, \"clash_hist\": %ld, \"fx_clash\": %ld, ", c.bits, c.draw_bits, c.max_draws, c.gt24, c.gt24_fast,
-          c.clash7_bits, c.clash7_stay, c.clash_hist_bits, c.fx_clash_bits);
+             "\"clash7_stay\": %ld, \"clash_hist\": %ld, \"fx_clash\": %ld, \"permuted\": %ld, ", c.bits, c.draw_bits, c.max_draws,
+          c.gt24, c.gt24_fast, c.clash7_bits, c.clash7_stay, c.clash_hist_bits, c.fx_clash_bits, c.permuted);
   const char* sep = "";
   for (const auto* v : {c.clash7_bpos, c.bucket7_bpos}) {
     fprintf(f, "\"%s\": [", v == c.clash7_bpos ? "clash7_bpos" : "bucket7_bpos");
@@ -161,7 +261,11 @@ inline void print(FILE* f, const std::vector<std::pair<std::string, const void*>
 
 #define P8_CENSUS_CM(T, m, y, c0, bp) census::p8_cm(T, m, y, c0, bp)
 #define P8_CENSUS_CM2(m, bpos) census::p8_cm2(m, bpos)
-#ifdef CENSUS_REVERSE
-#define P8_CM_ORDER(T, m, o, rnd, y, c0, bp, c1) do { const int r_ = census::p8_cm_reverse(T, m, o, rnd, y, c0, bp, c1); if (r_ >= 0) return r_; } while (0)
+#if defined(CENSUS_PERMUTE) || defined(CENSUS_REVERSE)
+#define P8_CM_ORDER(T, m, o, rnd, y, c0, bp, c1) do { const int r_ = census::p8_cm_order(T, m, o, rnd, y, c0, bp, c1); if (r_ >= 0) return r_; } while (0)
+#endif
+#ifdef CENSUS_PERMUTE
+#define P8_CM2_ORDER(m, o, y, bpos) do { const int r_ = census::p8_cm2_order(m, o, y, bpos); if (r_ >= 0) return r_; } while (0)
+#define FX_MAP_ORDER(S, id, o) do { if (census::fx_map_order(S, id, o)) return; } while (0)
 #endif
 #define FX_CENSUS_MAP(S, id) census::fx_map(S, id)

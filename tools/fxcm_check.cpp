@@ -9,7 +9,8 @@
 // LSTM feedback FXCM consumed (<prefix>.lstmfx.u32). With a dictionary the reference pretrains on a 5-byte header plus
 // the dictionary text (preprocessor.cpp:37-69) before the first coded bit; so does this tool.
 // With crc_out it writes one CRC32 per 4096 bits of its OWN codes (fixture generation once the run is green).
-// Built with -DCENSUS it also prints how often the coded bits reach the device-only clash path (tools/census.h).
+// Built with -DCENSUS it also prints how often the coded bits reach the device-only clash path (tools/census.h), and writes
+// the per-bit census log to the file the environment variable CENSUS_LOG names.
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -91,6 +92,7 @@ int main(int argc, char** argv) {
   }
 #ifdef CENSUS
   census::reset();
+  census::open_log(getenv("CENSUS_LOG"), true);
 #endif
 
   std::vector<uint16_t> want(2022);

@@ -8,7 +8,8 @@
 // A pretrain file holds the bytes the reference's Pretrain() saw before the first coded bit (5-byte header + dictionary
 // with '\n' -> ' ', preprocessor.cpp:37-69). With crc_out it writes one CRC32 per 4096 bits over its OWN 1591 codes.
 // first_slot/last_slot (0-based within the 1591) restrict the comparison while a sub-model range is being brought up.
-// Built with -DCENSUS it also prints how often the coded bits reach the device-only paths (tools/census.h).
+// Built with -DCENSUS it also prints how often the coded bits reach the device-only paths (tools/census.h), and writes the
+// per-bit census log to the file the environment variable CENSUS_LOG names.
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -75,7 +76,15 @@ int main(int argc, char** argv) {
     fprintf(stderr, "pretrained on %zu bytes\n", pre.size());
   }
 #ifdef CENSUS
+  const std::vector<std::pair<std::string, const void*>> maps = {
+      {"sparse", &S->sparse.cm}, {"sparse1", &S->sparse1.cm}, {"distance", &S->distance.cm}, {"record.cm", &S->record.cm},
+      {"record.cn", &S->record.cn}, {"record.co", &S->record.co}, {"record.cp", &S->record.cp}, {"record1.cm", &S->record1.cm},
+      {"record1.cn", &S->record1.cn}, {"record1.co", &S->record1.co}, {"record1.cq", &S->record1.cq},
+      {"record1.cp", &S->record1.cp}, {"word", &S->word.cm}, {"nest", &S->nest.cm}, {"indirect", &S->indirect.cm},
+      {"xml", &S->xml.cm}, {"order-n (history)", &S->cm}, {"text (history)", &S->text.map}, {"exe (history)", &S->exe.cm}};
   census::reset();
+  census::set_maps(maps);
+  census::open_log(getenv("CENSUS_LOG"), false);
 #endif
   std::vector<uint16_t> want(2022);
   std::vector<uint32_t> crcs;
@@ -118,11 +127,7 @@ int main(int argc, char** argv) {
   if (crc_out) { FILE* f = fopen(crc_out, "wb"); fwrite(crcs.data(), 4, crcs.size(), f); fclose(f); }
   if (unsupported) return 3;
 #ifdef CENSUS
-  census::print(stdout, {{"sparse", &S->sparse.cm}, {"sparse1", &S->sparse1.cm}, {"distance", &S->distance.cm}, {"record.cm", &S->record.cm},
-                         {"record.cn", &S->record.cn}, {"record.co", &S->record.co}, {"record.cp", &S->record.cp}, {"record1.cm", &S->record1.cm},
-                         {"record1.cn", &S->record1.cn}, {"record1.co", &S->record1.co}, {"record1.cq", &S->record1.cq},
-                         {"record1.cp", &S->record1.cp}, {"word", &S->word.cm}, {"nest", &S->nest.cm}, {"indirect", &S->indirect.cm},
-                         {"xml", &S->xml.cm}, {"order-n (history)", &S->cm}, {"text (history)", &S->text.map}, {"exe (history)", &S->exe.cm}});
+  census::print(stdout, maps);
 #endif
   printf("%s: %zu bytes, %zu mismatching bits (slots %d..%d)\n", bad_bits ? "FAIL" : "OK", n_bytes, bad_bits, first, last);
   return bad_bits ? 1 : 0;
