@@ -13,31 +13,33 @@ import numpy as np
 N_EXT = 2022
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
-LIB_PATH = os.environ.get("CMIXB200_LIB") or os.path.join(CSRC, "libcmixb200.so")   # CMIXB200_LIB: a profiling (tools/prof_build.py) or jitter (tests/test_schedule_jitter.py) build
+PRODUCT_LIB = os.path.join(CSRC, "libcmixb200.so")
+LIB_PATH = os.environ.get("CMIXB200_LIB") or PRODUCT_LIB   # CMIXB200_LIB: load a variant (profiling, jitter, census) instead
+UNITS = ["engine.cu", "fxcm_dev.cu", "paq8_dev.cu"]         # the three device programs, compiled side by side
 NVCC_COMPILE = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 NVCC_LINK = ["-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC"]
-NVCC_FLAGS = NVCC_COMPILE + ["-shared"]
 
 _lib = None
 
 
-def build_library(force=False):
-    """Compile cmix_b200/csrc/engine.cu for sm_90a into libcmixb200.so (in-tree)."""
+def build_library(force=False, defines=(), out_dir=None):
+    """Compile the UNITS for sm_90a and link them into libcmixb200.so; rebuilds when a source is newer. Returns its path.
+
+    By default this is the product, in csrc/. A variant (e.g. defines=["-DCMIXB200_JITTER"]) is built into its own out_dir."""
+    assert not defines or out_dir, "a variant build needs an out_dir of its own"
+    out_dir = out_dir or CSRC
+    lib, objs = os.path.join(out_dir, "libcmixb200.so"), [os.path.join(out_dir, u[:-3] + ".o") for u in UNITS]
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh", ".h"))]
     srcs.append(os.path.join(os.path.dirname(_HERE), "include", "cmixb200.h"))
-    if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(s) for s in srcs):
-        return LIB_PATH
-    units = ["engine.cu", "fxcm_dev.cu", "paq8_dev.cu"]
-    objs, jobs = [], []
-    for u in units:                                   # the three device programs compile side by side
-        obj = os.path.join(CSRC, u[:-3] + ".o")
-        objs.append(obj)
-        if force or not os.path.exists(obj) or any(os.path.getmtime(obj) < os.path.getmtime(s) for s in srcs):
-            jobs.append(subprocess.Popen(["nvcc"] + NVCC_COMPILE + ["-c", os.path.join(CSRC, u), "-o", obj]))
+    if not force and os.path.exists(lib) and all(os.path.getmtime(lib) >= os.path.getmtime(s) for s in srcs):
+        return lib
+    jobs = [subprocess.Popen(["nvcc"] + NVCC_COMPILE + list(defines) + ["-c", os.path.join(CSRC, u), "-o", obj])
+            for u, obj in zip(UNITS, objs)
+            if force or not os.path.exists(obj) or any(os.path.getmtime(obj) < os.path.getmtime(s) for s in srcs)]
     if any(j.wait() != 0 for j in jobs):
         raise RuntimeError("cmix_b200: nvcc failed")
-    subprocess.run(["nvcc"] + NVCC_LINK + objs + ["-o", LIB_PATH], check=True)
-    return LIB_PATH
+    subprocess.run(["nvcc"] + NVCC_LINK + objs + ["-o", lib], check=True)
+    return lib
 
 
 def load_library():

@@ -20,21 +20,16 @@ the first staying-bit slot clashes, three streams in one batch, and the device d
 import ctypes
 import json
 import os
-import subprocess
-import sys
 import time
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from gen_reach import STREAMS as REACH_STREAMS
 from gen_stress import STREAMS as STRESS_STREAMS
-from test_stress_data import _compile
+from harness import awkward, awkward_lock_step, batch, build_host_tool, child_jobs, even, expect, golden, round_trip, run_child, \
+    run_host_tools
 
-CSRC = os.path.join(ROOT, "cmix_b200", "csrc")
-UNITS = ["engine.cu", "fxcm_dev.cu", "paq8_dev.cu"]
 EXPORTS = ["cmixb200_census_attach", "cmixb200_census_read", "cmixb200_census_reset", "cmixb200_census_detach"]
 STRESS = ["stress_" + n for n in STRESS_STREAMS]
 REACH = ["reach_" + n for n in REACH_STREAMS]
@@ -49,13 +44,8 @@ HEAD = ["cap", "p8_bits", "fx_bits", "bit_checked", "bit_filled", "slot_checks",
         "first_bit", "first_map", "first_ctx", "first_byte", "first_cached", "first_hbm", "overflow"]
 
 
-def _load(name):
-    z = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
-    return {k: z[k] for k in z.files}
-
-
 def _lstmfx(name, g):
-    return _load(FX_FEEDBACK[name])["lstmfx"][:g["stream"].size * 8] if name in FX_FEEDBACK else g["lstmfx"]
+    return golden(FX_FEEDBACK[name])["lstmfx"][:g["stream"].size * 8] if name in FX_FEEDBACK else g["lstmfx"]
 
 
 def _staying(bp):
@@ -63,34 +53,16 @@ def _staying(bp):
 
 
 # ------------------------------------------------------------------------------------------------ host logs
-def _host_log(exe, tmp, label, stream, lstmfx=None):
-    """One run of paq8_check / fxcm_check built with -DCENSUS: (return code, output, CRCs per 4096 bits, census, log)."""
-    prefix = os.path.join(tmp, label)
-    stream.tofile(prefix + ".stream")
-    if lstmfx is not None:
-        lstmfx.tofile(prefix + ".lstmfx.u32")
-    env = dict(os.environ, CENSUS_LOG=prefix + ".log")
-    r = subprocess.run([exe, prefix, "-", str(stream.size), prefix + ".crc"], capture_output=True, text=True, env=env)
-    census = [json.loads(line[len("census "):]) for line in r.stdout.splitlines() if line.startswith("census ")]
-    crc = np.fromfile(prefix + ".crc", dtype=np.uint32) if os.path.exists(prefix + ".crc") else None
-    log = np.fromfile(prefix + ".log", dtype=np.uint32) if os.path.exists(prefix + ".log") else None
-    if log is not None and lstmfx is None:
-        log = log.reshape(-1, 3)
-    return r.returncode, r.stdout + r.stderr, crc, census[0] if census else None, log
-
-
 def _host_runs(tmp, defines=()):
-    """The host PAQ8 and FXCM builds over every fixture, in parallel: {("p8" | "fx", name): _host_log(...)}."""
-    p8 = _compile(tmp, "paq8_check", ["-ffp-contract=off", *defines])
-    fx = _compile(tmp, "fxcm_check", list(defines))
+    """The host PAQ8 and FXCM builds over every fixture, in parallel, with their per-bit logs: {("p8" | "fx", name): HostRun}."""
+    p8 = build_host_tool("paq8_check", tmp, ["-DCENSUS", *defines])
+    fx = build_host_tool("fxcm_check", tmp, ["-DCENSUS", *defines])
     jobs = {}
     for n in FIXTURES:
-        g = _load(n)
-        jobs[("p8", n)] = (p8, "p8_" + n, g["stream"], None)
-        jobs[("fx", n)] = (fx, "fx_" + n, g["stream"], _lstmfx(n, g))
-    with ThreadPoolExecutor(os.cpu_count() or 4) as ex:
-        futs = {k: ex.submit(_host_log, exe, tmp, label, s, l) for k, (exe, label, s, l) in jobs.items()}
-        return {k: f.result() for k, f in futs.items()}
+        g = golden(n)
+        jobs[("p8", n)] = (p8, tmp, "p8_" + n, g["stream"], None)
+        jobs[("fx", n)] = (fx, tmp, "fx_" + n, g["stream"], _lstmfx(n, g))
+    return run_host_tools(jobs, log=True)
 
 
 def _check_codes(runs, names):
@@ -99,7 +71,7 @@ def _check_codes(runs, names):
     for (m, n), (rc, out, crc, _, _) in sorted(runs.items()):
         if n not in names:
             continue
-        want = _load(n)["crc_p8" if m == "p8" else "crc_fx"]
+        want = golden(n)["crc_p8" if m == "p8" else "crc_fx"]
         if rc != 0:
             bad.append("%s %s: exit %d: %s" % (m, n, rc, out[-800:]))
         elif crc.size != want.size or not np.array_equal(crc, want):
@@ -147,10 +119,10 @@ def test_census_build_exports_and_the_product_does_not(census_lib):
 def test_host_logs_agree_with_the_census_totals(host_logs):
     bad = []
     for n in FIXTURES:
-        _, _, _, c8, log8 = host_logs[("p8", n)]
-        _, _, _, cfx, logfx = host_logs[("fx", n)]
+        c8, log8 = host_logs[("p8", n)].census, host_logs[("p8", n)].log
+        cfx, logfx = host_logs[("fx", n)].census, host_logs[("fx", n)].log
         assert log8 is not None and logfx is not None, "%s: a host run wrote no per-bit log" % n
-        assert log8.shape[0] == logfx.size == _load(n)["stream"].size * 8, n
+        assert log8.shape[0] == logfx.size == golden(n)["stream"].size * 8, n
         totals, maps, fx_maps, fx_clash = _totals(log8, logfx)
         for k, v in totals.items():
             if c8[k] != v:
@@ -170,7 +142,7 @@ def test_the_fixtures_discriminate(host_logs):
     differ from these logs somewhere."""
     rows, sums = [], {"rule": 0, "stay": 0, "hist": 0, "fx": 0, "serial_free": 0}
     for n in FIXTURES:
-        log8, logfx = host_logs[("p8", n)][4], host_logs[("fx", n)][4]
+        log8, logfx = host_logs[("p8", n)].log, host_logs[("fx", n)].log
         f = _p8_fields(log8)
         stay = np.array([_staying(b) for b in range(8)])[f["bp"]] == 1
         rule = int(np.sum(stay & (f["mask7"] != log8[:, 2])))      # staying bits where the slot and bucket rules disagree
@@ -192,159 +164,91 @@ def test_permuted_builds_match_the_reference(tmp_path_factory, seed):
     contexts of a map commute on these fixtures."""
     runs = _host_runs(str(tmp_path_factory.mktemp("census_permute")), ["-DCENSUS_PERMUTE=%#x" % seed])
     _check_codes(runs, FIXTURES)
-    unpermuted = [k for k, r in runs.items() if not r[3] or r[3]["permuted"] == 0]
+    unpermuted = [k for k, r in runs.items() if not r.census or r.census["permuted"] == 0]
     assert not unpermuted, "runs that permuted no map: %s" % unpermuted
-    print("seed %#x: %d PAQ8 and %d FXCM map-bits permuted" % (seed, sum(r[3]["permuted"] for k, r in runs.items() if k[0] == "p8"),
-                                                               sum(r[3]["permuted"] for k, r in runs.items() if k[0] == "fx")))
+    print("seed %#x: %d PAQ8 and %d FXCM map-bits permuted" % (seed, sum(r.census["permuted"] for k, r in runs.items() if k[0] == "p8"),
+                                                               sum(r.census["permuted"] for k, r in runs.items() if k[0] == "fx")))
 
 
 # ------------------------------------------------------------------------------------------------ the census build
 @pytest.fixture(scope="module")
 def census_lib(tmp_path_factory):
     """The library compiled with -DCMIXB200_CENSUS into this module's tmp dir."""
-    from cmix_b200.capi import NVCC_COMPILE, NVCC_LINK
-    out = tmp_path_factory.mktemp("census_lib")
-    objs, jobs = [], []
-    for u in UNITS:
-        obj = str(out / (u[:-3] + ".o"))
-        objs.append(obj)
-        jobs.append(subprocess.Popen(["nvcc"] + NVCC_COMPILE + ["-DCMIXB200_CENSUS", "-c", os.path.join(CSRC, u), "-o", obj]))
-    assert all(j.wait() == 0 for j in jobs), "nvcc failed on the census build"
-    lib = str(out / "libcmixb200_census.so")
-    subprocess.run(["nvcc"] + NVCC_LINK + objs + ["-o", lib], check=True)
-    return lib
+    from cmix_b200.capi import build_library
+    return build_library(defines=["-DCMIXB200_CENSUS"], out_dir=str(tmp_path_factory.mktemp("census_lib")))
 
 
 # ------------------------------------------------------------------------------------------------ GPU: child side
-class _Log:
-    """The census log of one predictor (census build only)."""
+class _Census:
+    """Stands in for the cmix_b200 module in the harness's schedules: each Predictor attaches a census log of n_bits on
+    creation and reads it back into `logs` when it closes (census build only). A failed read is kept in `errors`, not
+    raised from close(), so that it cannot replace the failure that brought a schedule into its `finally`."""
 
-    def __init__(self, lib, P, n_bits):
-        self.lib, self.P, self.n = lib, P, n_bits
-        self._call("attach", lib.cmixb200_census_attach(P._h, ctypes.c_uint(n_bits)))
+    def __init__(self, lib, n_bits):
+        import cmix_b200
+        census, self.logs, self.errors = self, [], []
 
-    def _call(self, what, rc):
-        if rc != 0:
-            raise RuntimeError("census %s: %s" % (what, self.lib.cmixb200_last_error().decode()))
+        def call(what, rc):
+            if rc != 0:
+                raise RuntimeError("census %s: %s" % (what, lib.cmixb200_last_error().decode()))
 
-    def read(self):
-        head = np.zeros(16, dtype=np.uint32)
-        p8 = np.zeros((self.n, 3), dtype=np.uint32)
-        fx = np.zeros(self.n, dtype=np.uint32)
-        self._call("read", self.lib.cmixb200_census_read(self.P._h, head.ctypes.data, p8.ctypes.data, fx.ctypes.data, ctypes.c_size_t(self.n)))
-        return {"head": head, "p8": p8, "fx": fx}
+        class Predictor(cmix_b200.Predictor):
+            def __init__(self, *args, **kw):
+                super().__init__(*args, **kw)
+                try:
+                    call("attach", lib.cmixb200_census_attach(self._h, ctypes.c_uint(n_bits)))
+                except BaseException:
+                    cmix_b200.Predictor.close(self)
+                    raise
 
-
-def _bulk(cm, lib, name, pieces):
-    from test_call_schedules import _expect
-    g = _load(name)
-    s, p = g["stream"], g["p"]
-    P = cm.Predictor(g["vocab"])
-    try:
-        log = _Log(lib, P, s.size * 8)
-        for a, b in pieces(s.size):
-            _expect("%s: bulk [%d,%d)" % (name, a, b), P.code_bytes(s[a:b]), p[a * 8:b * 8], a * 8)
-        return [log.read()]
-    finally:
-        P.close()
-
-
-def _lock(cm, lib, name, lo, hi):
-    """Bulk calls of 2048 bytes to byte lo, lock-step Predict()/Perceive() over [lo, hi), bulk calls to the end."""
-    from test_call_schedules import _expect, _lock_step
-    g = _load(name)
-    s, p = g["stream"], g["p"]
-    P = cm.Predictor(g["vocab"])
-    try:
-        log = _Log(lib, P, s.size * 8)
-        for a in range(0, lo, 2048):
-            b = min(a + 2048, lo)
-            _expect("%s: bulk [%d,%d)" % (name, a, b), P.code_bytes(s[a:b]), p[a * 8:b * 8], a * 8)
-        _lock_step(P, g, lo * 8, hi * 8, "%s: [%d,%d)" % (name, lo, hi))
-        for a in range(hi, s.size, 2048):
-            b = min(a + 2048, s.size)
-            _expect("%s: bulk [%d,%d) after lock-step" % (name, a, b), P.code_bytes(s[a:b]), p[a * 8:b * 8], a * 8)
-        return [log.read()]
-    finally:
-        P.close()
-
-
-def _batch(cm, lib, names):
-    import torch
-    from cmix_b200.capi import code_batch_device
-    from test_call_schedules import _expect
-    gs = [_load(x) for x in names]
-    n = min(g["stream"].size for g in gs)
-    preds = []
-    try:
-        for g in gs:
-            preds.append(cm.Predictor(g["vocab"]))
-        logs = [_Log(lib, P, n * 8) for P in preds]
-        dev = torch.device("cuda", 0)
-        d_bytes = [torch.from_numpy(g["stream"][:n].copy()).to(dev) for g in gs]
-        d_out = [torch.empty(n * 8, dtype=torch.float32, device=dev) for _ in gs]
-        code_batch_device(preds, d_bytes, n, None, None, d_out)
-        torch.cuda.synchronize()
-        for g, out, x in zip(gs, d_out, names):
-            _expect("batch of %s, %d bytes each: %s" % (list(names), n, x), out.cpu().numpy(), g["p"][:n * 8])
-        return [log.read() for log in logs]
-    finally:
-        for P in preds:
-            P.close()
-
-
-def _round_trip(cm, lib, name):
-    """Device encoder -> device decoder; the logs of both."""
-    from test_call_schedules import _expect, _first_bad_byte
-    g = _load(name)
-    s, p = g["stream"], g["p"]
-    enc = cm.Predictor(g["vocab"])
-    try:
-        log = _Log(lib, enc, s.size * 8)
-        enc.coder_begin(2 * s.size + 64)
-        _expect("%s: encoder" % name, enc.code_bytes(s), p)
-        archive = enc.coder_finish()
-        logs = [log.read()]
-    finally:
-        enc.close()
-    dec = cm.Predictor(g["vocab"])
-    try:
-        log = _Log(lib, dec, s.size * 8)
-        out = dec.decode_bytes(archive, s.size)
-        assert out.tobytes() == s.tobytes(), "%s, decoder: %s" % (name, _first_bad_byte(out, s))
-        return logs + [log.read()]
-    finally:
-        dec.close()
+            def close(self):
+                try:
+                    if getattr(self, "_h", None):
+                        head = np.zeros(16, dtype=np.uint32)
+                        p8 = np.zeros((n_bits, 3), dtype=np.uint32)
+                        fx = np.zeros(n_bits, dtype=np.uint32)
+                        call("read", lib.cmixb200_census_read(self._h, head.ctypes.data, p8.ctypes.data, fx.ctypes.data,
+                                                              ctypes.c_size_t(n_bits)))
+                        census.logs.append({"head": head, "p8": p8, "fx": fx})
+                except RuntimeError as e:
+                    census.errors.append(e)
+                finally:
+                    super().close()
+        self.Predictor = Predictor
 
 
 def _child(jobs_json, out_dir):
     """Run in a child interpreter with CMIXB200_LIB = the census build: each job is [schedule, args]; writes the logs of
     job j to out_dir/j.npz and prints one JSON line per job."""
     import cmix_b200
-    from test_reach import _awkward
     lib = cmix_b200.load_library()
-    for j, (sched, args) in enumerate(json.loads(jobs_json)):
-        t0 = time.perf_counter()
-        try:
-            if sched == "bulk":
-                logs = _bulk(cmix_b200, lib, args[0], lambda n: [(a, min(a + 2048, n)) for a in range(0, n, 2048)])
-            elif sched == "awkward":
-                logs = _bulk(cmix_b200, lib, args[0], lambda n: _awkward(0, n))
-            elif sched == "lock":
-                logs = _lock(cmix_b200, lib, *args)
-            elif sched == "batch":
-                logs = _batch(cmix_b200, lib, args)
-            elif sched == "round_trip":
-                logs = _round_trip(cmix_b200, lib, args[0])
-            else:
-                raise ValueError(sched)
-            np.savez(os.path.join(out_dir, "%d.npz" % j), **{"%s_%d" % (k, i): v for i, lg in enumerate(logs) for k, v in lg.items()})
-            msg = None
-        except BaseException as e:      # pytest.fail raises an exception outside pytest's Exception tree
-            msg = "%s: %s" % (type(e).__name__, e)
-        print(json.dumps({"sched": sched, "args": args, "s": round(time.perf_counter() - t0, 2), "fail": msg}), flush=True)
-        if msg and ("CUDA" in msg or "cuda" in msg):
-            break                        # the context may be gone: report, do not go on
+
+    def run(j, job):
+        sched, args = job
+        names = args if sched == "batch" else args[:1]
+        cm = _Census(lib, 8 * min(golden(n)["stream"].size for n in names))
+        if sched in ("bulk", "awkward"):
+            g = golden(args[0])
+            s, p = g["stream"], g["p"]
+            P = cm.Predictor(g["vocab"])
+            try:
+                for a, b in (even if sched == "bulk" else awkward)(0, s.size):
+                    expect("%s: bulk [%d,%d)" % (args[0], a, b), P.code_bytes(s[a:b]), p[a * 8:b * 8], a * 8)
+            finally:
+                P.close()
+        elif sched == "lock":
+            awkward_lock_step(cm, args[0], (args[1], args[2]), even)
+        elif sched == "batch":
+            batch(cm, args)
+        elif sched == "round_trip":
+            round_trip(cm, None, args[0])
+        else:
+            raise ValueError(sched)
+        if cm.errors:
+            raise cm.errors[0]
+        np.savez(os.path.join(out_dir, "%d.npz" % j), **{"%s_%d" % (k, i): v for i, lg in enumerate(cm.logs) for k, v in lg.items()})
+
+    child_jobs(json.loads(jobs_json), run)
 
 
 # ------------------------------------------------------------------------------------------------ GPU: parent side
@@ -390,46 +294,36 @@ def _compare(label, dev, host8, hostfx, lock=None):
 
 def _run(census_lib, host_logs, label, jobs, tmp, timeout=1500):
     """The jobs in a child interpreter; each job's logs compared with the host's. Fails with every difference."""
-    import gc
-    import torch
-    gc.collect()
-    torch.cuda.empty_cache()
     out_dir = str(tmp)
-    e = dict(os.environ, CMIXB200_LIB=census_lib)
-    e.setdefault("CMIXB200_PPMD_MB", "512")
-    code = "import sys; sys.path[:0] = sys.argv[1:4]; import test_device_census as m; m._child(sys.argv[4], sys.argv[5])"
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", code, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools"), ROOT, json.dumps(jobs), out_dir]
     t0 = time.perf_counter()
-    r = subprocess.run(cmd, env=e, cwd=ROOT, capture_output=True, text=True, timeout=timeout)
-    results = [json.loads(line) for line in r.stdout.splitlines() if line.startswith("{")]
+    results = run_child(census_lib, "test_device_census", "_child", [json.dumps(jobs), out_dir], timeout=timeout)
     fails = []
     print("\n%-12s %-44s %7s %7s %7s %9s %9s %9s" % ("schedule", "stream", "clash7", "hist", "fxcm", "copies", "sm words", "fills"))
     for j, x in enumerate(results):
+        sched, args = x["job"]
         if x["fail"]:
-            fails.append("%s %s: %s" % (x["sched"], x["args"], x["fail"]))
+            fails.append("%s %s: %s" % (sched, args, x["fail"]))
             continue
         z = np.load(os.path.join(out_dir, "%d.npz" % j))
-        names = {"batch": x["args"], "round_trip": [x["args"][0]] * 2}.get(x["sched"], [x["args"][0]])
+        names = {"batch": args, "round_trip": [args[0]] * 2}.get(sched, [args[0]])
         for i, name in enumerate(names):
             dev = {k: z["%s_%d" % (k, i)] for k in ("head", "p8", "fx")}
             n = dev["p8"].shape[0]
-            host8, hostfx = host_logs[("p8", name)][4][:n], host_logs[("fx", name)][4][:n]
-            what = "%s %s%s" % (x["sched"], name, " (decoder)" if x["sched"] == "round_trip" and i else "")
-            lock = (x["args"][1] * 8, x["args"][2] * 8) if x["sched"] == "lock" else None
+            host8, hostfx = host_logs[("p8", name)].log[:n], host_logs[("fx", name)].log[:n]
+            what = "%s %s%s" % (sched, name, " (decoder)" if sched == "round_trip" and i else "")
+            lock = (args[1] * 8, args[2] * 8) if sched == "lock" else None
             f, row = _compare(what, dev, host8, hostfx, lock)
             fails += f
             if row:
-                print("%-12s %-44s %7d %7d %7d %9d %9d %9d" % ((x["sched"], name + (" (decoder)" if x["sched"] == "round_trip" and i else "")) + row))
+                print("%-12s %-44s %7d %7d %7d %9d %9d %9d" % ((sched, name + (" (decoder)" if sched == "round_trip" and i else "")) + row))
     print("%s: %d runs in %.0f s" % (label, len(results), time.perf_counter() - t0))
-    assert r.returncode == 0, "%s: child failed:\n%s\n%s" % (label, r.stdout[-3000:], r.stderr[-3000:])
     assert not fails, "%s: %d differences:\n%s" % (label, len(fails), "\n".join(fails))
     assert len(results) == len(jobs), "%s: %d of %d runs reported" % (label, len(results), len(jobs))
 
 
 def _first_slot_clash(host_logs, name):
     """The byte of the first staying-bit slot clash of a fixture (host log)."""
-    f = _p8_fields(host_logs[("p8", name)][4])
+    f = _p8_fields(host_logs[("p8", name)].log)
     stay = np.array([_staying(b) for b in range(8)])[f["bp"]] == 1
     t = np.nonzero(stay & (f["mask7"] != 0))[0]
     assert t.size, "%s has no staying-bit slot clash" % name

@@ -7,37 +7,18 @@ without -fmad=false: if nothing is left for nvcc to contract, the two are the sa
 expansions of the IEEE intrinsics (__fdiv_rn, ...) and the explicit fused XM_DFMA; -fmad=false keeps them too. Needs
 nvcc, no GPU."""
 import os
-import re
 import subprocess
 from concurrent.futures import ThreadPoolExecutor
 
 import pytest
 
-from conftest import ROOT
-
-CSRC = os.path.join(ROOT, "cmix_b200", "csrc")
-UNITS = ["engine.cu", "fxcm_dev.cu", "paq8_dev.cu"]
-
-
-def _sass_by_function(cubin):
-    """{function name: its SASS} of a cubin (cuobjdump -sass)."""
-    text = subprocess.run(["cuobjdump", "-sass", cubin], check=True, capture_output=True, text=True).stdout
-    funcs, name = {}, None
-    for line in text.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            funcs[name] = []
-        elif name is not None:
-            ins = re.sub(r"/\*.*?\*/", "", line).strip()      # drop addresses and encodings: compare the instructions
-            if ins:
-                funcs[name].append(ins)
-    return {k: "\n".join(v) for k, v in funcs.items()}
+from cmix_b200.capi import NVCC_COMPILE, UNITS
+from harness import CSRC, sass_by_function
 
 
 def _first_difference(a, b):
     """(function, first differing SASS line with and without -fmad=false) of two cubins, or None."""
-    fa, fb = _sass_by_function(a), _sass_by_function(b)
+    fa, fb = sass_by_function(a), sass_by_function(b)
     for name in sorted(set(fa) | set(fb)):
         la, lb = fa.get(name, "").splitlines(), fb.get(name, "").splitlines()
         for x, y in zip(la + [""] * len(lb), lb + [""] * len(la)):
@@ -48,7 +29,6 @@ def _first_difference(a, b):
 
 @pytest.mark.timeout(900)
 def test_device_units_are_the_same_with_fmad_false(tmp_path):
-    from cmix_b200.capi import NVCC_COMPILE
     flags = [f for f in NVCC_COMPILE if f != "-lineinfo"]     # line tables are not code
 
     def compile_(unit, extra):

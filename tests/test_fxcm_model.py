@@ -5,41 +5,29 @@ unmodified reference (tools/make_fxcm_golden.py): every one of the 431 exported 
 (one CRC32 per 4096 bits). GPU (-m gpu): the same fixtures through the device kernels with PPMD, LSTM and FXCM all
 resident, so the LSTM feedback FXCM consumes is the device's own."""
 import os
-import subprocess
 import zlib
 
 import numpy as np
 import pytest
 
 from conftest import ROOT, Golden
+from harness import build_host_tool, cm, golden, pretrain_buffer, run_host_tool  # noqa: F401  (cm: fixture)
 
 FIXTURES = ["fxcm_text", "fxcm_bin", "fxcm_wrt"]
 
 
-def _load(name):
-    z = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
-    return {k: z[k] for k in z.files}
-
-
 @pytest.fixture(scope="module")
 def fxcm_check(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("fx") / "fxcm_check")
-    subprocess.run(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "cmix_b200", "csrc"),
-                    os.path.join(ROOT, "tools", "fxcm_check.cpp"), "-o", exe], check=True)
-    return exe
+    return build_host_tool("fxcm_check", str(tmp_path_factory.mktemp("fx")))
 
 
 @pytest.mark.parametrize("name", FIXTURES)
 def test_host_build_matches_reference_codes(fxcm_check, dict_path, tmp_path, name):
-    g = _load(name)
+    g = golden(name)
     use_dict = bool(g["dictionary"][0])
-    prefix = str(tmp_path / "d")
-    g["stream"].tofile(prefix + ".stream")
-    g["lstmfx"].tofile(prefix + ".lstmfx.u32")
-    crc_out = prefix + ".crc"
-    r = subprocess.run([fxcm_check, prefix, dict_path if use_dict else "-", str(g["stream"].size), crc_out], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    got = np.fromfile(crc_out, dtype=np.uint32)
+    r = run_host_tool(fxcm_check, str(tmp_path), "d", g["stream"], g["lstmfx"], dictionary=dict_path if use_dict else None)
+    assert r.rc == 0, r.out
+    got = r.crc
     bad = np.nonzero(got != g["crc"])[0]
     assert got.size == g["crc"].size and bad.size == 0, "first differing 4096-bit block: %s" % (bad[:1],)
 
@@ -59,13 +47,6 @@ def test_tables_are_the_reference_tables():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-@pytest.fixture(scope="module")
-def cm():
-    import cmix_b200
-    cmix_b200.load_library()
-    return cmix_b200
-
-
 def _device_code_crcs(cm, g, dictionary=None, pretrain=None, piece=2048):
     P = cm.Predictor(g["vocab"], dictionary_path=dictionary)
     if pretrain is not None:
@@ -89,7 +70,7 @@ def _device_code_crcs(cm, g, dictionary=None, pretrain=None, piece=2048):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["fxcm_text", "fxcm_bin"])
 def test_device_fxcm_chain_matches_reference_codes(cm, name):
-    g = _load(name)
+    g = golden(name)
     got, first = _device_code_crcs(cm, g)
     assert np.array_equal(first, g["first_codes"]), "codes of the first 64 bits"
     bad = np.nonzero(got != g["crc"])[0]
@@ -99,9 +80,8 @@ def test_device_fxcm_chain_matches_reference_codes(cm, name):
 @pytest.mark.gpu
 def test_device_fxcm_with_dictionary_and_pretraining(cm, dict_path):
     """cmix -c english.dic: WRT code words in the stream, Pretrain() over header + dictionary before the first bit."""
-    g = _load("fxcm_wrt")
-    d = open(dict_path, "rb").read()
-    pre = bytes([0, (len(d) >> 24) & 255, (len(d) >> 16) & 255, (len(d) >> 8) & 255, len(d) & 255]) + d.replace(b"\n", b" ")
+    g = golden("fxcm_wrt")
+    pre = pretrain_buffer(dict_path)
     n = 2048                                                   # 3 CRC blocks... keep the GPU test short: pretraining dominates
     g = dict(g); g["stream"] = g["stream"][:n]
     got, first = _device_code_crcs(cm, g, dictionary=dict_path, pretrain=pre)

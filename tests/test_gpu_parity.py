@@ -9,18 +9,12 @@ import numpy as np
 import pytest
 
 from conftest import ROOT, Golden, port_replay, synthetic_streams
+from harness import cm, golden  # noqa: F401  (cm: fixture)
 
 pytestmark = pytest.mark.gpu
 
 TOL = 0.0   # probabilities must match bit for bit; the spec's tolerance is 1e-5
 REPLAY_ALL = ("fxcm", "paq8")   # tests driven by synthetic code streams replay the big model groups instead of running them
-
-
-@pytest.fixture(scope="module")
-def cm():
-    import cmix_b200
-    cmix_b200.load_library()        # raises if the sm_90a library is missing: no fallback
-    return cmix_b200
 
 
 def _check_intermediates(P, g, nb):
@@ -197,7 +191,7 @@ def test_resident_ppmd_lock_step(cm, golden_text):
 def test_resident_ppmd_distributions_on_device(cm, name):
     """The device build of ppmd_model.h against fixtures from reference dumps (one CRC per byte)."""
     import zlib
-    g = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
+    g = golden(name)
     n = min(12000, g["stream"].size)
     import torch
     P = cm.Predictor(g["vocab"], replay=REPLAY_ALL)
@@ -283,7 +277,7 @@ def test_reference_dump_of_synthetic_text(cm):
     """The reference's Predict() over 2 KB of synthetic enwik-shaped text (gen_synth seed 0xE9E80002, `cmix -n` stream;
     tools/make_ref_goldens.py) is matched exactly by the complete resident predictor, and so is its bpc."""
     from gen_synth import synth_text
-    d = np.load(os.path.join(ROOT, "tests", "golden", "synth2000.npz"))
+    d = golden("synth2000")
     assert d["stream"][5:].tobytes() == synth_text(2000, 0xE9E80002)
     P = cm.Predictor(d["vocab"])
     p = P.code_bytes(d["stream"])

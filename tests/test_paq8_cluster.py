@@ -6,28 +6,14 @@ and the model CTA's state over exactly. Checked against the reference's dumps (t
 every bit and all 2 022 codes of the first 64 bits) at tolerance 0, after each call: the probabilities, the PAQ8 codes the
 bulk kernel wrote per bit and the codes handed to the next Predict() (State::codes after a bulk call). Also: an error
 raised by the model CTA (a JPEG header) still reaches the host when the mixer CTA writes back its part of the state."""
-import os
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from harness import cm, golden  # noqa: F401  (cm: fixture)
 
 pytestmark = pytest.mark.gpu
 
 DBG_EXT_GEN, DBG_EXT_BIT = 10, 11
-
-
-def _load(name):
-    z = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
-    return {k: z[k] for k in z.files}
-
-
-@pytest.fixture(scope="module")
-def cm():
-    import cmix_b200
-    cmix_b200.load_library()
-    return cmix_b200
 
 
 def _same(what, got, want):
@@ -37,7 +23,7 @@ def _same(what, got, want):
 
 
 def test_ring_depths_lock_step_and_bulk(cm):
-    g = _load("full_text")
+    g = golden("full_text")
     s, first, p_ref = g["stream"], g["first_codes"], g["p"]
     bits = np.unpackbits(s)
     assert first.shape[0] >= 64
@@ -72,7 +58,7 @@ def test_ring_depths_lock_step_and_bulk(cm):
 
 def test_model_cta_error_reaches_the_host(cm):
     """A JPEG header in the third bulk call: the model CTA raises the sticky error, the mixer CTA owns the rest of the state."""
-    g = _load("full_text")
+    g = golden("full_text")
     text = g["stream"][:400].copy()
     jpeg = np.frombuffer(bytes([0xFF, 0xD8, 0xFF, 0xE0, 0x00, 0x10]) + b"JFIF\x00\x01\x01\x00\x00\x01\x00\x01\x00\x00", dtype=np.uint8)
     P = cm.Predictor(np.ones(256, dtype=np.uint8))

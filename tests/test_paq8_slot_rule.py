@@ -9,35 +9,29 @@ clashes walks serially (p8_number / cm_mix). CPU only:
     context taking the draw of its in-order rank, as the device's lanes do) reproduces the reference's PAQ8 codes.
 tests/test_device_census.py generalises the second test to a seeded random order on every bit, in the history maps and
 FXCM's maps too (-DCENSUS_PERMUTE), and pins the device's per-bit verdicts to this census."""
-import os
-from concurrent.futures import ThreadPoolExecutor
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from gen_stress import STREAMS
-from test_stress_data import _compile, _host_run, _load
+from harness import build_host_tool, golden, run_host_tools
 
 STRESS = ["stress_" + n for n in STREAMS]
 BASELINE = ["full_text", "full_bin"]
 
 
 def _runs(tmp, exe, names):
-    with ThreadPoolExecutor(os.cpu_count() or 4) as ex:
-        futs = {n: ex.submit(_host_run, exe, tmp, n, _load(n)["stream"]) for n in names}
-        return {n: f.result() for n, f in futs.items()}
+    return run_host_tools({n: (exe, tmp, n, golden(n)["stream"]) for n in names})
 
 
 @pytest.fixture(scope="module")
 def census_runs(tmp_path_factory):
     tmp = str(tmp_path_factory.mktemp("slot_census"))
-    return _runs(tmp, _compile(tmp, "paq8_check", ["-ffp-contract=off"]), BASELINE + STRESS)
+    return _runs(tmp, build_host_tool("paq8_check", tmp, ["-DCENSUS"]), BASELINE + STRESS)
 
 
 def test_staying_bits_clash_only_in_the_stress_fixtures(census_runs):
     rows = BASELINE + STRESS
-    census = {n: census_runs[n][3] for n in rows}
+    census = {n: census_runs[n].census for n in rows}
     assert all(c is not None for c in census.values()), "a host run printed no census"
     lines = ["%-16s %-7s" % ("7-slot clash bits", "rule") + "".join("%8s" % ("bpos %d" % b) for b in range(8))]
     for n in rows:
@@ -57,12 +51,12 @@ def test_staying_bits_clash_only_in_the_stress_fixtures(census_runs):
 
 def test_reverse_order_on_clash_free_staying_bits_matches_the_reference(tmp_path_factory):
     tmp = str(tmp_path_factory.mktemp("slot_reverse"))
-    exe = _compile(tmp, "paq8_check", ["-ffp-contract=off", "-DCENSUS_REVERSE"])
+    exe = build_host_tool("paq8_check", tmp, ["-DCENSUS", "-DCENSUS_REVERSE"])
     runs = _runs(tmp, exe, BASELINE + STRESS)
     for n in BASELINE + STRESS:
-        rc, out, crc, _ = runs[n]
+        rc, out, crc = runs[n][:3]
         assert rc == 0, "%s:\n%s" % (n, out[-2000:])
-        want = _load(n)["crc_p8"]
+        want = golden(n)["crc_p8"]
         bad = np.nonzero(crc != want[:crc.size])[0]
         assert crc.size == want.size and bad.size == 0, "%s: %d CRC blocks, expected %d; first differing 4096-bit block %s" % (
             n, crc.size, want.size, bad[:1])

@@ -6,38 +6,17 @@ one CRC-32 per byte of the 256-float distribution PPMD::ByteUpdate leaves, ppmd.
 and with the full distributions stored in the golden dumps. The device build of the same header is
 checked by tests/test_gpu_parity.py.
 """
-import ctypes
-import os
-import subprocess
 import zlib
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def ppmd_host(tmp_path_factory):
-    so = tmp_path_factory.mktemp("ppmd") / "libppmd_host.so"
-    subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC",
-                    os.path.join(ROOT, "tools", "ppmd_host.cpp"), "-o", str(so)], check=True)
-    lib = ctypes.CDLL(str(so))
-    lib.ppmd_host_run.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint]
-    lib.ppmd_host_run.restype = ctypes.c_int
-
-    def run(stream, vocab, arena_mb=64):
-        stream = np.ascontiguousarray(stream, dtype=np.uint8)
-        vocab = np.ascontiguousarray(vocab, dtype=np.uint8)
-        out = np.zeros((stream.size, 256), dtype=np.float32)
-        rc = lib.ppmd_host_run(stream.ctypes.data, stream.size, vocab.ctypes.data, out.ctypes.data, arena_mb)
-        return rc, out
-    return run
+from harness import golden, ppmd_host  # noqa: F401  (ppmd_host: fixture)
 
 
 @pytest.mark.parametrize("name", ["ppmd_text40k", "ppmd_bin6k", "ppmd_rand", "ppmd_rep", "ppmd_dic"])
 def test_distributions_match_the_reference_dump(ppmd_host, name):
-    g = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
+    g = golden(name)
     rc, out = ppmd_host(g["stream"], g["vocab"])
     assert rc == 0
     got = np.array([zlib.crc32(out[t].tobytes()) for t in range(out.shape[0])], dtype=np.uint32)

@@ -16,15 +16,13 @@ lock-step stretch across the bytes each stream targets; three streams in one bat
 round trip."""
 import os
 import zlib
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from gen_reach import STREAMS, coded_stream
-from test_ppmd_model import ppmd_host  # noqa: F401  (fixture)
-from test_stress_data import _check_host, _compile, _host_run
+from harness import awkward_lock_step, batch, build_host_tool, check_host, cm, code_in_pieces, even, golden, ppmd_arena, \
+    ppmd_host, round_trip, run_host_tools  # noqa: F401  (cm, ppmd_arena, ppmd_host: fixtures)
 
 NAMES = list(STREAMS)
 GATE_CAP = 65536 if os.environ.get("CMIXB200_SLOW") == "1" else 8192
@@ -53,8 +51,7 @@ ALLOWED = [
 
 
 def _fixture(name):
-    z = np.load(os.path.join(ROOT, "tests", "golden", "reach_" + name + ".npz"))
-    return {k: z[k] for k in z.files}
+    return golden("reach_" + name)
 
 
 # ------------------------------------------------------------------------------------------------ CPU
@@ -62,30 +59,28 @@ def _fixture(name):
 def host_runs(tmp_path_factory):
     """The host PAQ8 and FXCM builds over every reach fixture, in parallel."""
     tmp = str(tmp_path_factory.mktemp("reach"))
-    p8 = _compile(tmp, "paq8_check", ["-ffp-contract=off"])
-    fx = _compile(tmp, "fxcm_check")
+    p8 = build_host_tool("paq8_check", tmp, ["-DCENSUS"])
+    fx = build_host_tool("fxcm_check", tmp, ["-DCENSUS"])
     jobs = {}
     for name in NAMES:
         g = _fixture(name)
-        jobs[("p8", name)] = (p8, "p8_" + name, g["stream"], None)
-        jobs[("fx", name)] = (fx, "fx_" + name, g["stream"], g["lstmfx"])
-    with ThreadPoolExecutor(os.cpu_count() or 4) as ex:
-        futs = {k: ex.submit(_host_run, exe, tmp, label, s, l) for k, (exe, label, s, l) in jobs.items()}
-        return {k: f.result() for k, f in futs.items()}
+        jobs[("p8", name)] = (p8, tmp, "p8_" + name, g["stream"], None)
+        jobs[("fx", name)] = (fx, tmp, "fx_" + name, g["stream"], g["lstmfx"])
+    return run_host_tools(jobs)
 
 
 @pytest.mark.parametrize("name", NAMES)
 def test_paq8_host_build_matches_reference_codes(host_runs, name):
-    _check_host(host_runs[("p8", name)], _fixture(name)["crc_p8"], "reach_%s, PAQ8" % name)
+    check_host(host_runs[("p8", name)], _fixture(name)["crc_p8"], "reach_%s, PAQ8" % name)
 
 
 @pytest.mark.parametrize("name", NAMES)
 def test_fxcm_host_build_matches_reference_codes(host_runs, name):
-    _check_host(host_runs[("fx", name)], _fixture(name)["crc_fx"], "reach_%s, FXCM" % name)
+    check_host(host_runs[("fx", name)], _fixture(name)["crc_fx"], "reach_%s, FXCM" % name)
 
 
 @pytest.mark.parametrize("name", NAMES)
-def test_ppmd_host_build_matches_reference_distributions(ppmd_host, name):  # noqa: F811
+def test_ppmd_host_build_matches_reference_distributions(ppmd_host, name):
     g = _fixture(name)
     rc, out = ppmd_host(g["stream"], g["vocab"])
     assert rc == 0
@@ -141,70 +136,18 @@ def test_every_line_of_the_shared_models_runs_on_some_fixture():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-# the bytes each stream is built to reach: lock-step runs over [marker + lo, marker + hi)
-TARGETS = {"english": (b"+\r\n", -8, 24), "europe": (b"travaux", -4, 20), "xml": (b"<![CDATA[", -4, 52),
-           "x86": (b"\x0f\x3a", -4, 28), "dbase": (b"visual foxpro table\n", 18, 70),
-           "bmp": (b"\x28\x00\x00\x00\x10\x00\x00\x00", 24, 48), "fxwiki": (b"PPQ", -4, 36)}
-
-
-def _target(name, s):
-    marker, lo, hi = TARGETS[name]
-    at = s.tobytes().find(marker)
-    assert at >= 0, "reach_%s: marker %r not in the stream" % (name, marker)
-    return at + lo, min(at + hi, s.size)
-
-
-@pytest.fixture(autouse=True)
-def _ppmd_arena(monkeypatch):
-    if "CMIXB200_PPMD_MB" not in os.environ:
-        monkeypatch.setenv("CMIXB200_PPMD_MB", "512")      # three full predictors must fit in 80 GB
-
-
-@pytest.fixture(scope="module")
-def cm():
-    import cmix_b200
-    cmix_b200.load_library()
-    return cmix_b200
-
-
 @pytest.mark.gpu
 @pytest.mark.timeout(900)
 @pytest.mark.parametrize("name", NAMES)
 def test_everything_resident_in_bulk(cm, name):
     """Bulk calls of 2048 bytes (a bulk call's debug codes cover its last 2048-byte piece): every Predict(), every FXCM
     and PAQ8 code and every PPMD distribution equal the reference's."""
-    from test_stress_data import _mismatch_report
     g = _fixture(name)
-    s = g["stream"]
     P = cm.Predictor(g["vocab"])
-    ps, exts, ppmd_crc = [], [], []
     try:
-        for off in range(0, s.size, 2048):
-            part = s[off:off + 2048]
-            ps.append(P.code_bytes(part))
-            exts.append(P.debug_fetch(10, (part.size * 8, 2022), np.uint16))
-            rows = P.debug_fetch(8, (part.size, 256), np.float32)
-            ppmd_crc += [zlib.crc32(rows[t].tobytes()) for t in range(part.size)]
+        code_in_pieces(P, g, even(0, g["stream"].size))
     finally:
         P.close()
-    ext = np.concatenate(exts)
-    crc_fx = np.array([zlib.crc32(np.ascontiguousarray(ext[b:b + 4096, :431]).tobytes()) for b in range(0, ext.shape[0], 4096)], dtype=np.uint32)
-    crc_p8 = np.array([zlib.crc32(np.ascontiguousarray(ext[b:b + 4096, 431:]).tobytes()) for b in range(0, ext.shape[0], 4096)], dtype=np.uint32)
-    report = _mismatch_report(name, g, np.concatenate(ps), crc_fx, crc_p8, ext[:64], np.array(ppmd_crc, dtype=np.uint32))
-    if report:
-        pytest.fail(report.replace("stress_", "reach_", 1), pytrace=False)
-
-
-def _awkward(lo, hi):
-    """Pieces of [lo, hi): 1, 129, 7, 1000, 333 bytes, then the rest."""
-    out = []
-    for n in (1, 129, 7, 1000, 333):
-        if lo < hi:
-            out.append((lo, min(lo + n, hi)))
-            lo = out[-1][1]
-    if lo < hi:
-        out.append((lo, hi))
-    return out
 
 
 @pytest.mark.gpu
@@ -213,19 +156,7 @@ def _awkward(lo, hi):
 def test_lock_step_across_the_target_in_awkward_pieces(cm, name):
     """Bulk calls of awkward sizes up to the bytes the stream targets, lock-step Predict()/Perceive() across them, then
     bulk calls of awkward sizes to the end."""
-    from test_call_schedules import _expect, _lock_step
-    g = _fixture(name)
-    s, p = g["stream"], g["p"]
-    lo, hi = _target(name, s)
-    P = cm.Predictor(g["vocab"])
-    try:
-        for a, b in _awkward(0, lo):
-            _expect("reach_%s: bulk [%d,%d)" % (name, a, b), P.code_bytes(s[a:b]), p[a * 8:b * 8], a * 8)
-        _lock_step(P, g, lo * 8, hi * 8, "reach_%s: lock-step [%d,%d)" % (name, lo, hi))
-        for a, b in _awkward(hi, s.size):
-            _expect("reach_%s: bulk [%d,%d) after lock-step" % (name, a, b), P.code_bytes(s[a:b]), p[a * 8:b * 8], a * 8)
-    finally:
-        P.close()
+    awkward_lock_step(cm, "reach_" + name)
 
 
 @pytest.mark.gpu
@@ -233,25 +164,7 @@ def test_lock_step_across_the_target_in_awkward_pieces(cm, name):
 @pytest.mark.parametrize("names", [("english", "europe", "xml"), ("x86", "dbase", "bmp"), ("fxwiki", "english", "x86")])
 def test_three_streams_in_one_batch(cm, names):
     """Three streams of the same length side by side in one code_batch_device call (three predictors fit in 80 GB)."""
-    import torch
-    from cmix_b200.capi import code_batch_device
-    from test_call_schedules import _expect
-    gs = [_fixture(n) for n in names]
-    n = min(g["stream"].size for g in gs)
-    preds = []
-    try:
-        for g in gs:
-            preds.append(cm.Predictor(g["vocab"]))
-        dev = torch.device("cuda", 0)
-        d_bytes = [torch.from_numpy(g["stream"][:n].copy()).to(dev) for g in gs]
-        d_out = [torch.empty(n * 8, dtype=torch.float32, device=dev) for _ in gs]
-        code_batch_device(preds, d_bytes, n, None, None, d_out)
-        torch.cuda.synchronize()
-        for g, out, name in zip(gs, d_out, names):
-            _expect("batch of %s, %d bytes each: reach_%s" % (list(names), n, name), out.cpu().numpy(), g["p"][:n * 8])
-    finally:
-        for P in preds:
-            P.close()
+    batch(cm, ["reach_" + n for n in names])
 
 
 @pytest.mark.gpu
@@ -260,21 +173,4 @@ def test_three_streams_in_one_batch(cm, names):
 def test_device_round_trip(cm, port, name):
     """The device coder writes the archive the host coder writes over the reference's probabilities; the device decoder
     gets the stream back."""
-    from test_call_schedules import _expect, _first_bad_byte, _host_archive
-    g = _fixture(name)
-    s, p = g["stream"], g["p"]
-    enc = cm.Predictor(g["vocab"])
-    try:
-        enc.coder_begin(2 * s.size + 64)
-        _expect("reach_%s: encoder" % name, enc.code_bytes(s), p)
-        archive = enc.coder_finish()
-    finally:
-        enc.close()
-    want = _host_archive(port, p, np.unpackbits(s))
-    assert archive == want, "reach_%s: device archive differs from the host encoder's: %s" % (name, _first_bad_byte(archive, want))
-    dec = cm.Predictor(g["vocab"])
-    try:
-        out = dec.decode_bytes(archive, s.size)
-    finally:
-        dec.close()
-    assert out.tobytes() == s.tobytes(), "reach_%s, decoder: %s" % (name, _first_bad_byte(out, s))
+    round_trip(cm, port, "reach_" + name)

@@ -10,95 +10,56 @@ CPU (-m "not gpu"): the host builds of PAQ8, FXCM and PPMD against those CRCs; t
 census (tools/census.h) of how often the fixtures reach each device-only path, next to the same census of full_text/full_bin.
 GPU (-m gpu, tolerance 0): every fixture with everything resident, in bulk calls of awkward sizes; lock-step then bulk; three
 classes in one batch; and a device encoder -> device decoder round trip."""
-import json
-import os
-import subprocess
 import zlib
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from gen_stress import STREAMS, coded_stream
-from test_ppmd_model import ppmd_host  # noqa: F401  (fixture)
+from harness import batch, build_host_tool, check_host, cm, code_in_pieces, expect, golden, lock_step, ppmd_arena, ppmd_host, \
+    round_trip, run_host_tools, stress_pieces  # noqa: F401  (cm, ppmd_arena, ppmd_host: fixtures)
 
 NAMES = list(STREAMS)
 # the existing whole-predictor fixtures, for comparison in the census (FXCM's LSTM feedback comes from fxcm_*.npz: same streams)
 BASELINE = {"full_text": "fxcm_text", "full_bin": "fxcm_bin"}
 
 
-def _load(name):
-    z = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
-    return {k: z[k] for k in z.files}
-
-
 def _fixture(name):
-    return _load("stress_" + name)
+    return golden("stress_" + name)
 
 
 # ------------------------------------------------------------------------------------------------ CPU
-def _compile(tmp, tool, extra=()):
-    exe = os.path.join(tmp, tool)
-    subprocess.run(["g++", "-O2", "-std=c++17", "-DCENSUS", *extra, "-I", os.path.join(ROOT, "cmix_b200", "csrc"), "-I",
-                    os.path.join(ROOT, "tools"), os.path.join(ROOT, "tools", tool + ".cpp"), "-o", exe], check=True)
-    return exe
-
-
-def _host_run(exe, tmp, label, stream, lstmfx=None):
-    """One run of paq8_check / fxcm_check (built with -DCENSUS): (return code, output, CRCs per 4096 bits, census)."""
-    prefix = os.path.join(tmp, label)
-    stream.tofile(prefix + ".stream")
-    if lstmfx is not None:
-        lstmfx.tofile(prefix + ".lstmfx.u32")
-    r = subprocess.run([exe, prefix, "-", str(stream.size), prefix + ".crc"], capture_output=True, text=True)
-    census = [json.loads(line[len("census "):]) for line in r.stdout.splitlines() if line.startswith("census ")]
-    crc = np.fromfile(prefix + ".crc", dtype=np.uint32) if os.path.exists(prefix + ".crc") else None
-    return r.returncode, r.stdout + r.stderr, crc, census[0] if census else None
-
-
 @pytest.fixture(scope="module")
 def host_runs(tmp_path_factory):
     """The host PAQ8 and FXCM builds over every stress fixture and over full_text / full_bin, in parallel."""
     tmp = str(tmp_path_factory.mktemp("stress"))
-    p8 = _compile(tmp, "paq8_check", ["-ffp-contract=off"])
-    fx = _compile(tmp, "fxcm_check")
+    p8 = build_host_tool("paq8_check", tmp, ["-DCENSUS"])
+    fx = build_host_tool("fxcm_check", tmp, ["-DCENSUS"])
     jobs = {}
     for name in NAMES:
         g = _fixture(name)
-        jobs[("p8", name)] = (p8, "p8_" + name, g["stream"], None)
-        jobs[("fx", name)] = (fx, "fx_" + name, g["stream"], g["lstmfx"])
+        jobs[("p8", name)] = (p8, tmp, "p8_" + name, g["stream"], None)
+        jobs[("fx", name)] = (fx, tmp, "fx_" + name, g["stream"], g["lstmfx"])
     for name, fx_name in BASELINE.items():
-        s, f = _load(name)["stream"], _load(fx_name)
+        s, f = golden(name)["stream"], golden(fx_name)
         assert np.array_equal(f["stream"][:s.size], s)
-        jobs[("p8", name)] = (p8, "p8_" + name, s, None)
-        jobs[("fx", name)] = (fx, "fx_" + name, s, f["lstmfx"][:s.size * 8])
-    with ThreadPoolExecutor(os.cpu_count() or 4) as ex:
-        futs = {k: ex.submit(_host_run, exe, tmp, label, s, l) for k, (exe, label, s, l) in jobs.items()}
-        return {k: f.result() for k, f in futs.items()}
-
-
-def _check_host(run, want, what):
-    rc, out, crc, _ = run
-    assert rc != 3, "%s: the stream trips PAQ8's image / audio / JPEG gate:\n%s" % (what, out[-2000:])
-    assert rc == 0, "%s:\n%s" % (what, out[-2000:])
-    bad = np.nonzero(crc != want[:crc.size])[0]
-    assert crc.size == want.size and bad.size == 0, "%s: %d CRC blocks, expected %d; first differing 4096-bit block %s" % (
-        what, crc.size, want.size, bad[:1])
+        jobs[("p8", name)] = (p8, tmp, "p8_" + name, s, None)
+        jobs[("fx", name)] = (fx, tmp, "fx_" + name, s, f["lstmfx"][:s.size * 8])
+    return run_host_tools(jobs)
 
 
 @pytest.mark.parametrize("name", NAMES)
 def test_paq8_host_build_matches_reference_codes(host_runs, name):
-    _check_host(host_runs[("p8", name)], _fixture(name)["crc_p8"], "stress_%s, PAQ8" % name)
+    check_host(host_runs[("p8", name)], _fixture(name)["crc_p8"], "stress_%s, PAQ8" % name)
 
 
 @pytest.mark.parametrize("name", NAMES)
 def test_fxcm_host_build_matches_reference_codes(host_runs, name):
-    _check_host(host_runs[("fx", name)], _fixture(name)["crc_fx"], "stress_%s, FXCM" % name)
+    check_host(host_runs[("fx", name)], _fixture(name)["crc_fx"], "stress_%s, FXCM" % name)
 
 
 @pytest.mark.parametrize("name", NAMES)
-def test_ppmd_host_build_matches_reference_distributions(ppmd_host, name):  # noqa: F811
+def test_ppmd_host_build_matches_reference_distributions(ppmd_host, name):
     g = _fixture(name)
     rc, out = ppmd_host(g["stream"], g["vocab"])
     assert rc == 0
@@ -123,7 +84,7 @@ def test_census_reaches_every_device_only_path(host_runs):
     """Counts, per fixture, the coded bits that take each device-only path (the device's own rule applied by the host build,
     tools/census.h). The stress fixtures together must reach every path, and every map family's clash fallback."""
     rows = list(BASELINE) + NAMES
-    census = {(m, n): host_runs[(m, n)][3] for m in ("p8", "fx") for n in rows}
+    census = {(m, n): host_runs[(m, n)].census for m in ("p8", "fx") for n in rows}
     assert all(c is not None for c in census.values()), "a host run printed no census"
     lines = ["%-38s" % "coded bits" + "".join("%11s" % n for n in rows) + "%11s" % "stress"]
     lines.append("%-38s" % "bits" + "".join("%11d" % census[("p8", n)]["bits"] for n in rows)
@@ -152,85 +113,28 @@ def test_census_reaches_every_device_only_path(host_runs):
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-@pytest.fixture(autouse=True)
-def _ppmd_arena(monkeypatch):
-    if "CMIXB200_PPMD_MB" not in os.environ:
-        monkeypatch.setenv("CMIXB200_PPMD_MB", "512")      # three full predictors must fit in 80 GB
-
-
-@pytest.fixture(scope="module")
-def cm():
-    import cmix_b200
-    cmix_b200.load_library()
-    return cmix_b200
-
-
-def _pieces(n):
-    """1, 129 and 1000 bytes, then pieces of at most 2000 (a bulk call's debug codes cover its last 2048-byte piece only)."""
-    sizes = [1, 129, 1000]
-    while sum(sizes) < n:
-        sizes.append(min(2000, n - sum(sizes)))
-    return sizes
-
-
-def _mismatch_report(name, g, p, crc_fx, crc_p8, first, ppmd_crc):
-    """Every way the device run differs from the fixture, each with its first bit / byte / 4096-bit block."""
-    out = []
-    d = np.nonzero(p.view(np.uint32) != g["p"].view(np.uint32))[0]
-    if d.size:
-        k = int(d[0])
-        out.append("Predict(): first differing bit %d (byte %d, block %d; %.9g vs %.9g; %d bits differ)"
-                   % (k, k // 8, k // 4096, p[k], g["p"][k], d.size))
-    bad = np.argwhere(first != g["first_codes"])
-    if bad.size:
-        out.append("codes of the first 64 bits: first differing (bit, slot) %s" % (bad[0].tolist(),))
-    for what, got, want in (("FXCM", crc_fx, g["crc_fx"]), ("PAQ8", crc_p8, g["crc_p8"])):
-        b = np.nonzero(got != want)[0]
-        if b.size:
-            out.append("%s codes: first differing block %d (bits %d..%d)" % (what, b[0], b[0] * 4096, b[0] * 4096 + 4095))
-    b = np.nonzero(ppmd_crc != g["ppmd_crc"])[0]
-    if b.size:
-        out.append("PPMD distribution: first differing after byte %d" % b[0])
-    return ("stress_%s: " % name + "; ".join(out)) if out else None
-
-
 @pytest.mark.gpu
 @pytest.mark.timeout(900)
 @pytest.mark.parametrize("name", NAMES)
 def test_everything_resident_in_awkward_pieces(cm, name):
     """Bulk calls of 1, 129, 1000, ... bytes put sub-chunk boundaries inside runs, records and samples."""
     g = _fixture(name)
-    s = g["stream"]
     P = cm.Predictor(g["vocab"])
-    ps, exts, ppmd_crc = [], [], []
     try:
-        off = 0
-        for n in _pieces(s.size):
-            ps.append(P.code_bytes(s[off:off + n]))
-            exts.append(P.debug_fetch(10, (n * 8, 2022), np.uint16))
-            rows = P.debug_fetch(8, (n, 256), np.float32)
-            ppmd_crc += [zlib.crc32(rows[t].tobytes()) for t in range(n)]
-            off += n
+        code_in_pieces(P, g, stress_pieces(g["stream"].size))
     finally:
         P.close()
-    ext = np.concatenate(exts)
-    crc_fx = np.array([zlib.crc32(np.ascontiguousarray(ext[b:b + 4096, :431]).tobytes()) for b in range(0, ext.shape[0], 4096)], dtype=np.uint32)
-    crc_p8 = np.array([zlib.crc32(np.ascontiguousarray(ext[b:b + 4096, 431:]).tobytes()) for b in range(0, ext.shape[0], 4096)], dtype=np.uint32)
-    report = _mismatch_report(name, g, np.concatenate(ps), crc_fx, crc_p8, ext[:64], np.array(ppmd_crc, dtype=np.uint32))
-    if report:
-        pytest.fail(report, pytrace=False)
 
 
 @pytest.mark.gpu
 @pytest.mark.timeout(900)
 @pytest.mark.parametrize("name", ["zeros", "random", "pcm16"])
 def test_lock_step_then_bulk(cm, name):
-    from test_call_schedules import _expect, _lock_step
     g = _fixture(name)
     P = cm.Predictor(g["vocab"])
     try:
-        _lock_step(P, g, 0, 64 * 8, "stress_%s: lock-step [0,64)" % name)
-        _expect("stress_%s: lock-step [0,64), bulk [64,%d)" % (name, g["stream"].size), P.code_bytes(g["stream"][64:]), g["p"][64 * 8:], 64 * 8)
+        lock_step(P, g, 0, 64 * 8, "stress_%s: lock-step [0,64)" % name)
+        expect("stress_%s: lock-step [0,64), bulk [64,%d)" % (name, g["stream"].size), P.code_bytes(g["stream"][64:]), g["p"][64 * 8:], 64 * 8)
     finally:
         P.close()
 
@@ -239,26 +143,7 @@ def test_lock_step_then_bulk(cm, name):
 @pytest.mark.timeout(900)
 def test_three_classes_in_one_batch(cm):
     """records, zeros (every context draws) and the mixed stream side by side in one code_batch_device call."""
-    import torch
-    from cmix_b200.capi import code_batch_device
-    from test_call_schedules import _expect
-    names = ["records", "zeros", "mixed"]
-    gs = [_fixture(n) for n in names]
-    n = min(g["stream"].size for g in gs)
-    preds = []
-    try:
-        for g in gs:
-            preds.append(cm.Predictor(g["vocab"]))
-        dev = torch.device("cuda", 0)
-        d_bytes = [torch.from_numpy(g["stream"][:n].copy()).to(dev) for g in gs]
-        d_out = [torch.empty(n * 8, dtype=torch.float32, device=dev) for _ in gs]
-        code_batch_device(preds, d_bytes, n, None, None, d_out)
-        torch.cuda.synchronize()
-        for g, out, name in zip(gs, d_out, names):
-            _expect("batch of %s, %d bytes each: stress_%s" % (names, n, name), out.cpu().numpy(), g["p"][:n * 8])
-    finally:
-        for P in preds:
-            P.close()
+    batch(cm, ["stress_records", "stress_zeros", "stress_mixed"])
 
 
 @pytest.mark.gpu
@@ -266,21 +151,4 @@ def test_three_classes_in_one_batch(cm):
 def test_device_round_trip_of_the_mixed_stream(cm, port):
     """The device coder writes the archive the host coder writes over the reference's probabilities; the device decoder
     gets the stream back."""
-    from test_call_schedules import _expect, _first_bad_byte, _host_archive
-    g = _fixture("mixed")
-    s, p = g["stream"], g["p"]
-    enc = cm.Predictor(g["vocab"])
-    try:
-        enc.coder_begin(2 * s.size + 64)
-        _expect("stress_mixed: encoder", enc.code_bytes(s), p)
-        archive = enc.coder_finish()
-    finally:
-        enc.close()
-    want = _host_archive(port, p, np.unpackbits(s))
-    assert archive == want, "stress_mixed: device archive differs from the host encoder's: %s" % _first_bad_byte(archive, want)
-    dec = cm.Predictor(g["vocab"])
-    try:
-        out = dec.decode_bytes(archive, s.size)
-    finally:
-        dec.close()
-    assert out.tobytes() == s.tobytes(), "stress_mixed, decoder: %s" % _first_bad_byte(out, s)
+    round_trip(cm, port, "stress_mixed")

@@ -29,11 +29,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "cmix_b200", "csrc")
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
-# tool -> (source, extra flags, the shared headers it measures)
+# host tool -> the g++ flags every build of it takes, the tests' and this report's
+HOST_FLAGS = {"paq8_check": ["-ffp-contract=off"], "fxcm_check": [], "ppmd_host": ["-ffp-contract=off"]}
+# tool -> (host tool, extra flags of its executable here, the shared headers it measures)
 TOOLS = {
-    "paq8": ("paq8_check.cpp", ["-ffp-contract=off"], ["paq8_model.h", "paq8_predict.h", "paq8_text.h", "paq8_top.h"]),
-    "fxcm": ("fxcm_check.cpp", [], ["fxcm_model.h", "fxcm_text.h"]),
-    "ppmd": ("ppmd_host.cpp", ["-ffp-contract=off", "-DPPMD_HOST_MAIN"], ["ppmd_model.h"]),
+    "paq8": ("paq8_check", [], ["paq8_model.h", "paq8_predict.h", "paq8_text.h", "paq8_top.h"]),
+    "fxcm": ("fxcm_check", [], ["fxcm_model.h", "fxcm_text.h"]),
+    "ppmd": ("ppmd_host", ["-DPPMD_HOST_MAIN"], ["ppmd_model.h"]),
 }
 DEFAULT_CAP = 40000
 
@@ -48,13 +50,18 @@ def _fixtures(names=None):
     return out
 
 
+def gxx(tool, out, flags=()):
+    """The g++ command that builds tools/<tool>.cpp into `out` with its HOST_FLAGS and `flags`."""
+    return ["g++", "-std=c++17", *HOST_FLAGS[tool], *flags, "-I", CSRC, "-I", os.path.join(ROOT, "tools"),
+            os.path.join(ROOT, "tools", tool + ".cpp"), "-o", out]
+
+
 def _build(work, tool):
     src, flags, _ = TOOLS[tool]
     d = os.path.join(work, "build", tool)
     os.makedirs(d)
     obj, exe = os.path.join(d, tool + ".o"), os.path.join(d, tool)
-    subprocess.run(["g++", "-O1", "--coverage", "-std=c++17", *flags, "-I", CSRC, "-c", os.path.join(ROOT, "tools", src),
-                    "-o", obj], check=True)
+    subprocess.run(gxx(src, obj, ["-O1", "--coverage", *flags, "-c"]), check=True)
     subprocess.run(["g++", "--coverage", obj, "-o", exe], check=True)
     return d, exe
 

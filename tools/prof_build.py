@@ -1,18 +1,18 @@
 #!/usr/bin/env python
-"""Build a profiling variant of the library (-DP8_PROF -DFX_PROF: per-phase cycle counters in the producer kernels) next to
-the product library and print where a bit's time goes. Never used by the product path, the tests or bench.py.
+"""Build a profiling variant of the library (-DP8_PROF -DFX_PROF: per-phase cycle counters in the producer kernels) into
+cmix_b200/csrc/prof/ and print where a bit's time goes. Never used by the product path, the tests or bench.py.
 
     python tools/prof_build.py build            # here (nvcc cross-compiles)
     python tools/prof_build.py run [n_bytes]    # on the GPU box: CMIXB200_LIB=<prof lib> is set by this script
 """
 import ctypes
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "cmix_b200", "csrc")
-PROF_LIB = os.path.join(CSRC, "libcmixb200_prof.so")
+PROF_DIR = os.path.join(CSRC, "prof")
+PROF_LIB = os.path.join(PROF_DIR, "libcmixb200.so")
 
 
 # PAQ8's slots. 0-11 add up to the model CTA's bit, 16-19 to the mixer CTA's. From 24 on: inside a byte the time a warp spent
@@ -81,16 +81,9 @@ def paq8_classes(a):
 
 def build():
     sys.path.insert(0, ROOT)
-    from cmix_b200.capi import NVCC_COMPILE, NVCC_LINK
-    objs, jobs = [], []
-    for u in ["engine.cu", "fxcm_dev.cu", "paq8_dev.cu"]:
-        obj = os.path.join(CSRC, u[:-3] + "_prof.o")
-        objs.append(obj)
-        jobs.append(subprocess.Popen(["nvcc"] + NVCC_COMPILE + ["-DP8_PROF", "-DFX_PROF", "-c", os.path.join(CSRC, u), "-o", obj]))
-    if any(j.wait() != 0 for j in jobs):
-        raise SystemExit("nvcc failed")
-    subprocess.run(["nvcc"] + NVCC_LINK + objs + ["-o", PROF_LIB], check=True)
-    print(PROF_LIB)
+    from cmix_b200.capi import build_library
+    os.makedirs(PROF_DIR, exist_ok=True)
+    print(build_library(force=True, defines=["-DP8_PROF", "-DFX_PROF"], out_dir=PROF_DIR))
 
 
 def run(n_bytes):
