@@ -118,6 +118,7 @@ class Predictor:
         _check(self._lib, self._lib.cmixb200_create_ex(v.ctypes.data, d, int(device), mask, ctypes.byref(h)), "create")
         self._h = h
         self.device = device
+        self.replay = tuple(replay)
 
     def close(self):
         if getattr(self, "_h", None):

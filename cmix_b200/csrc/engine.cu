@@ -829,6 +829,19 @@ int RunPipelined(cmixb200_predictor** preds, int n_streams, const u8* const* d_b
   // only waits for its own producers and the groups drift apart instead of moving in lock-step waves.
   static const int kGroup = getenv("CMIXB200_GROUP") ? atoi(getenv("CMIXB200_GROUP")) : 8;
   const int gsz = kGroup > 0 ? kGroup : n_streams;
+  // With a group resident the mixer stages every slot from ext_gen, and only the resident group writes its own. The
+  // replayed group's slots take the caller's codes, or 0.5 (0xFFFF) when the call has none (cmixb200.h), on the stream
+  // the mixer runs on, before its first launch. With every group replayed the mixer reads the caller's codes directly.
+  if (!pretrain)
+    for (int s = 0; s < n_streams; ++s) {
+      cmixb200_predictor* P = preds[s];
+      const auto [first, last] = ReplayedSlots(P);
+      if (!(P->d_fx || P->d_p8) || last == first) continue;
+      const cudaStream_t st = preds[s - s % gsz]->s_mix;
+      const size_t pitch = N_EXT * sizeof(u16), width = (last - first) * sizeof(u16), rows = n_bytes * 8;
+      if (d_ext && d_ext[s]) CK(cudaMemcpy2DAsync(P->d_ext_gen.p + first, pitch, d_ext[s] + first, pitch, width, rows, cudaMemcpyDeviceToDevice, st));
+      else CK(cudaMemset2DAsync(P->d_ext_gen.p + first, pitch, 0xFF, width, rows, st));
+    }
   for (size_t k = 0; k < n_sub; ++k)
     for (int g0 = 0; g0 < n_streams; g0 += gsz) {
       const int cnt = n_streams - g0 < gsz ? n_streams - g0 : gsz;

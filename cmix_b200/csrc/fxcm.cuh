@@ -426,8 +426,7 @@ __device__ void fx_mixer_bit(FxShared& sh, u32 t, int y, const short* x_prev, in
 }
 
 // Bulk: cluster b (CTAs 2b, 2b+1) serves stream b of the launch group. The mixer CTA writes ext[t][0..430] for every bit t
-// of the sub-chunk (the codes the model holds BEFORE perceiving bit t) and, when a.ext_replay is given, copies the
-// non-resident PAQ8 slots next to them.
+// of the sub-chunk (the codes the model holds BEFORE perceiving bit t).
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FX_THREADS, 1) fxcm_kernel(const ChunkArgs* __restrict__ args_all) { jit_entry(JK_FXCM);
   extern __shared__ __align__(16) unsigned char fx_raw[];
   FxShared& sh = *reinterpret_cast<FxShared*>(fx_raw);
@@ -451,7 +450,6 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(FX_THREADS, 1) fxcm_
       if (!a.pretrain) {
         u16* out = a.ext_gen + (size_t)t * N_EXT;
         for (int k = tid; k < fx::N_OUT; k += FX_THREADS) out[k] = sh.S.codes[k];
-        if (a.ext_replay && !a.paq8) for (int k = fx::N_OUT + tid; k < N_EXT; k += FX_THREADS) out[k] = a.ext_replay[(size_t)t * N_EXT + k];
       }
       const int y = (a.bytes[t >> 3] >> (7 - (t & 7))) & 1;
       fx_mixer_bit(sh, t, y, t == 0 ? sh.S.in1 : sh.u.mx.ring[(t - 1) % FX_RING].in1, tid);

@@ -197,7 +197,8 @@ struct ChunkArgs {
   u32 n_bytes;
   u32 pretrain;                 // 1: Pretrain() semantics (models + contexts only)
   // resident FXCM / PAQ8 (fxcm.cuh, paq8.cuh): they write their 12-bit codes into ext_gen ([n_bytes*8][N_EXT]); `ext` above is
-  // then == ext_gen. Slots of a model that is NOT resident are copied from ext_replay (the caller's replayed codes) when given.
+  // then == ext_gen. ext_replay is the caller's codes (or null); no kernel reads it: the host stages the slots of a model
+  // that is NOT resident into ext_gen before the mixer runs (RunPipelined).
   fx::State* fx;                // null = FXCM replayed
   void* paq8;                   // null = PAQ8 replayed
   u16* ext_gen;

@@ -39,9 +39,11 @@ int cmixb200_create(const uint8_t vocab[256], const char* dictionary_path, int d
                     cmixb200_predictor** out);
 void cmixb200_destroy(cmixb200_predictor*);
 
-/* Same, choosing which of the big model groups are REPLAYED instead of device resident (test and A/B hook: a replayed
- * group costs no HBM and takes its outputs from cmixb200_feed_external_* / the `ext` / `ppmd` arguments of the bulk calls;
- * without them its inputs carry p = 0.5). cmixb200_create == replay_mask 0 == everything that is resident is used. */
+/* Same, choosing which of the big model groups are REPLAYED instead of device resident: a replayed group costs no HBM
+ * and takes its codes from cmixb200_feed_external_bit / the `ext` argument of the bulk calls; a bulk call without `ext`
+ * gives its inputs p = 0.5. CMIXB200_REPLAY_PAQ8 is how image, PCM WAV audio and JPEG data are coded (the resident PAQ8
+ * returns CMIXB200_ERR_UNSUPPORTED there). Predictors of one batch must replay the same groups, and decode_bytes needs
+ * every group resident. cmixb200_create == replay_mask 0 == everything that is resident is used. */
 enum { CMIXB200_REPLAY_FXCM = 1, CMIXB200_REPLAY_PAQ8 = 2 };
 int cmixb200_create_ex(const uint8_t vocab[256], const char* dictionary_path, int device, unsigned replay_mask,
                        cmixb200_predictor** out);

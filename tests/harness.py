@@ -83,10 +83,13 @@ def expect(schedule, got, want, first_bit=0):
                     % (schedule, first_bit + k, (first_bit + k) // 8, got[k], want[k], d.size, got.size), pytrace=False)
 
 
-def lock_step(P, g, lo, hi, schedule):
-    """Predict()/Perceive(bit) over bits [lo, hi) of the fixture's stream, each Predict() checked as it comes."""
+def lock_step(P, g, lo, hi, schedule, feed=None):
+    """Predict()/Perceive(bit) over bits [lo, hi) of the fixture's stream, each Predict() checked as it comes. feed(P, t)
+    runs before the Predict() of bit t (the replayed groups' codes: feed_external_bit)."""
     bits = np.unpackbits(g["stream"])
     for t in range(lo, hi):
+        if feed is not None:
+            feed(P, t)
         expect(schedule + ", lock-step", np.float32([P.Predict()]), g["p"][t:t + 1], t)
         P.Perceive(int(bits[t]))
 
@@ -100,6 +103,52 @@ def host_archive(port, p, bits):
     n = port.op_enc_finish(e, buf.ctypes.data, buf.size)
     port.op_enc_destroy(e)
     return buf[:n].tobytes()
+
+
+def host_decode(P, archive, n_bytes, before_predict=None):
+    """Decoder::Decode (reference src/coder/decoder.cpp:3-39) on the host over lock-step Predict()/Perceive().
+    before_predict(P, t) runs before the Predict() of bit t (the replayed groups' codes: feed_external_bit)."""
+    arch = bytes(archive)
+    pos = 0
+
+    def read():
+        nonlocal pos
+        b = arch[pos] if pos < len(arch) else 0
+        pos += 1
+        return b
+    x1, x2, x = 0, 0xFFFFFFFF, 0
+    for _ in range(4):
+        x = ((x << 8) + read()) & 0xFFFFFFFF
+    out = bytearray()
+    t = 0
+    for _ in range(n_bytes):
+        byte = 0
+        for _ in range(8):
+            if before_predict is not None:
+                before_predict(P, t)
+            p = int(np.float32(1.0) + np.float32(65534.0) * np.float32(P.Predict()))
+            rng = x2 - x1
+            xmid = (x1 + (rng >> 16) * p + (((rng & 0xFFFF) * p) >> 16)) & 0xFFFFFFFF
+            if x <= xmid:
+                bit, x2 = 1, xmid
+            else:
+                bit, x1 = 0, (xmid + 1) & 0xFFFFFFFF
+            P.Perceive(bit)
+            t += 1
+            while ((x1 ^ x2) & 0xFF000000) == 0:
+                x1 = (x1 << 8) & 0xFFFFFFFF
+                x2 = ((x2 << 8) + 255) & 0xFFFFFFFF
+                x = ((x << 8) + read()) & 0xFFFFFFFF
+            byte = byte * 2 + bit
+        out.append(byte)
+    return bytes(out)
+
+
+def code_crcs(ext):
+    """CRC32 per 4096 bits of [bits][2022] codes over the 431 FXCM slots and over the 1591 PAQ8 slots (the fixtures'
+    crc_fx, crc_p8)."""
+    return [np.array([zlib.crc32(np.ascontiguousarray(ext[t:t + 4096, lo:hi]).tobytes()) for t in range(0, len(ext), 4096)],
+                     dtype=np.uint32) for lo, hi in ((0, 431), (431, 2022))]
 
 
 def first_bad_byte(got, want):
@@ -176,17 +225,19 @@ def onsets(ctx):
 
 
 # ------------------------------------------------------------------------------------------------ GPU schedules
-def code_in_pieces(P, g, pieces, after=None):
+def code_in_pieces(P, g, pieces, after=None, ext=None):
     """Bulk calls over the (a, b) byte pieces, in order from byte 0, then every way the run differs from the fixture's
     prefix it covers, each with its first bit, byte or block: Predict(), the first 64 code rows, the FXCM and PAQ8 code
-    CRCs per 4096 bits and, where the fixture has them, the PPMD distribution CRCs per byte. after(P, a, b) runs after each
-    call. Returns {"p", "crc_fx", "crc_p8"}."""
+    CRCs per 4096 bits and, where the fixture has them, the PPMD distribution CRCs per byte. ext ([bits][2022] codes of the
+    whole stream) is passed to each call for the replayed groups; the codes checked are those the mixer staged, which are
+    the caller's own when no group is resident. after(P, a, b) runs after each call. Returns {"p", "crc_fx", "crc_p8"}."""
     s = g["stream"]
     ps, exts, ppmd_crc = [], [], []
+    resident = set(P.replay) != {"fxcm", "paq8"}
     for a, b in pieces:
         assert b - a <= MAX_PIECE, "%s: piece [%d,%d) is longer than the debug fetch covers" % (g["name"], a, b)
-        ps.append(P.code_bytes(s[a:b]))
-        exts.append(P.debug_fetch(DBG_EXT_GEN, ((b - a) * 8, 2022), np.uint16))
+        ps.append(P.code_bytes(s[a:b], None if ext is None else ext[a * 8:b * 8]))
+        exts.append(P.debug_fetch(DBG_EXT_GEN, ((b - a) * 8, 2022), np.uint16) if resident else ext[a * 8:b * 8])
         if "ppmd_crc" in g:
             rows = P.debug_fetch(DBG_PPMD_ROWS, (b - a, 256), np.float32)
             ppmd_crc += [zlib.crc32(rows[t].tobytes()) for t in range(b - a)]
@@ -194,11 +245,7 @@ def code_in_pieces(P, g, pieces, after=None):
             after(P, a, b)
     p, ext = np.concatenate(ps), np.concatenate(exts)
     nb = p.size
-
-    def crc(lo, hi):
-        return np.array([zlib.crc32(np.ascontiguousarray(ext[t:t + 4096, lo:hi]).tobytes()) for t in range(0, nb, 4096)],
-                        dtype=np.uint32)
-    got = {"p": p, "crc_fx": crc(0, 431), "crc_p8": crc(431, 2022)}
+    got = dict(zip(("crc_fx", "crc_p8"), code_crcs(ext)), p=p)
     out = []
     d = np.nonzero(p.view(np.uint32) != g["p"][:nb].view(np.uint32))[0]
     if d.size:
@@ -347,6 +394,49 @@ def check_host(run, want, what):
     bad = np.nonzero(run.crc != want[:run.crc.size])[0]
     assert run.crc.size == want.size and bad.size == 0, "%s: %d CRC blocks, expected %d; first differing 4096-bit block %s" % (
         what, run.crc.size, want.size, bad[:1])
+
+
+# ------------------------------------------------------------------------------------------------ the reference's codes
+ORACLE_DUMP = os.path.join(ROOT, "oracle", "_ref", "oracle_dump")
+JFIF = bytes([0xFF, 0xD8, 0xFF, 0xE0, 0x00, 0x10]) + b"JFIF\x00\x01\x01\x00\x00\x01\x00\x01\x00\x00"
+
+
+def reference_inputs():
+    """{name: (the file the reference codes, its cmix mode, coded bytes to dump)}: each fixture's recipe (its make_*
+    tool), and jfif_text, full_text's first 400 bytes with a JFIF header at byte 103, which has no fixture."""
+    from gen_reach import STREAMS as REACH, generate as reach
+    from gen_synth import synth_text
+    from gen_wav import STREAMS as WAV, generate as wav
+    out = {name: (wav(name, n, seed), mode, n) for name, (n, seed, mode) in WAV.items() if name.startswith("wav_")}
+    out["full_text"] = (np.frombuffer(synth_text(40000)[:12000], dtype=np.uint8), "n", 6144)
+    out["reach_fxwiki"] = (reach("fxwiki", *REACH["fxwiki"]), "n", REACH["fxwiki"][0])
+    text = golden("full_text")["stream"][:400]
+    jfif = np.concatenate([text[:103], np.frombuffer(JFIF, dtype=np.uint8), text[103:]])
+    out["jfif_text"] = (jfif, "n", jfif.size + 5)
+    return out
+
+
+def reference_dumps(out_dir, names=None):
+    """{name: oracle_io.Dump} of oracle_dump at level 1 (Predict(), every bit's 2022 codes, PPMD's distribution after every
+    byte) over reference_inputs() (by default all of them), the dumps side by side, written under out_dir."""
+    from oracle_io import Dump
+    if not os.path.exists(ORACLE_DUMP):
+        pytest.fail("%s is missing: __graft_entry__.build() compiles it from the reference's sources" % ORACLE_DUMP,
+                    pytrace=False)
+    inputs = reference_inputs()
+    names = list(names or inputs)
+
+    def dump(name):
+        data, mode, n = inputs[name]
+        src, prefix = os.path.join(out_dir, name + ".bin"), os.path.join(out_dir, name)
+        data.tofile(src)
+        r = subprocess.run([ORACLE_DUMP, "dump", mode, src, prefix, "1", str(n)], capture_output=True, text=True)
+        assert r.returncode == 0, "oracle_dump over %s:\n%s" % (name, (r.stdout + r.stderr)[-2000:])
+        return Dump(prefix)
+    # a reference process holds about 6 GB of models: four at a time, the longest streams first
+    with ThreadPoolExecutor(min(len(names), 4)) as ex:
+        futs = {name: ex.submit(dump, name) for name in sorted(names, key=lambda x: -inputs[x][2])}
+        return {name: futs[name].result() for name in names}
 
 
 # ------------------------------------------------------------------------------------------------ child interpreters

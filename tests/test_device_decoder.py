@@ -10,6 +10,8 @@ import time
 import numpy as np
 import pytest
 
+from harness import host_decode
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "full_text.npz")
 
@@ -18,40 +20,6 @@ def test_symbol_is_exported():
     from cmix_b200.capi import load_library
     lib = load_library()
     assert hasattr(lib, "cmixb200_decode_bytes")
-
-
-def host_decode(P, archive, n_bytes):
-    """Decoder::Decode (reference src/coder/decoder.cpp:3-39) on the host over lock-step Predict()/Perceive()."""
-    arch = bytes(archive)
-    pos = 0
-
-    def read():
-        nonlocal pos
-        b = arch[pos] if pos < len(arch) else 0
-        pos += 1
-        return b
-    x1, x2, x = 0, 0xFFFFFFFF, 0
-    for _ in range(4):
-        x = ((x << 8) + read()) & 0xFFFFFFFF
-    out = bytearray()
-    for _ in range(n_bytes):
-        byte = 0
-        for _ in range(8):
-            p = int(np.float32(1.0) + np.float32(65534.0) * np.float32(P.Predict()))
-            rng = x2 - x1
-            xmid = (x1 + (rng >> 16) * p + (((rng & 0xFFFF) * p) >> 16)) & 0xFFFFFFFF
-            if x <= xmid:
-                bit, x2 = 1, xmid
-            else:
-                bit, x1 = 0, (xmid + 1) & 0xFFFFFFFF
-            P.Perceive(bit)
-            while ((x1 ^ x2) & 0xFF000000) == 0:
-                x1 = (x1 << 8) & 0xFFFFFFFF
-                x2 = ((x2 << 8) + 255) & 0xFFFFFFFF
-                x = ((x << 8) + read()) & 0xFFFFFFFF
-            byte = byte * 2 + bit
-        out.append(byte)
-    return bytes(out)
 
 
 @pytest.mark.gpu
