@@ -309,7 +309,7 @@ def batch(cm, names, n=None):
 
 def round_trip(cm, port, name, n_decode=None):
     """Device encoder -> archive equal to the host encoder's over the reference's probabilities (port=None: not compared)
-    -> device decoder over the first n_decode bytes."""
+    -> device decoder over the first n_decode bytes. Returns the device's archive."""
     g = golden(name)
     s, p = g["stream"], g["p"]
     enc = cm.Predictor(g["vocab"])
@@ -329,6 +329,7 @@ def round_trip(cm, port, name, n_decode=None):
     finally:
         dec.close()
     assert out.tobytes() == s[:n].tobytes(), "%s, decoder: %s" % (name, first_bad_byte(out, s[:n]))
+    return archive
 
 
 def wav_until_unsupported(cm, name):
@@ -416,27 +417,68 @@ def reference_inputs():
     return out
 
 
-def reference_dumps(out_dir, names=None):
-    """{name: oracle_io.Dump} of oracle_dump at level 1 (Predict(), every bit's 2022 codes, PPMD's distribution after every
-    byte) over reference_inputs() (by default all of them), the dumps side by side, written under out_dir."""
+def reference_dumps(out_dir, names=None, level=1, inputs=None):
+    """{name: oracle_io.Dump} of oracle_dump at `level` (1: Predict(), every bit's 2022 codes, PPMD's distribution after
+    every byte; 2 adds every bit's layer-0 inputs, mixer outputs and selectors and the LSTM's distribution after every
+    byte) over `inputs` ({name: (file, cmix mode, coded bytes to dump)}; by default reference_inputs()), by default all of
+    them, the dumps side by side, written under out_dir."""
     from oracle_io import Dump
     if not os.path.exists(ORACLE_DUMP):
         pytest.fail("%s is missing: __graft_entry__.build() compiles it from the reference's sources" % ORACLE_DUMP,
                     pytrace=False)
-    inputs = reference_inputs()
+    inputs = inputs or reference_inputs()
     names = list(names or inputs)
 
     def dump(name):
         data, mode, n = inputs[name]
         src, prefix = os.path.join(out_dir, name + ".bin"), os.path.join(out_dir, name)
         data.tofile(src)
-        r = subprocess.run([ORACLE_DUMP, "dump", mode, src, prefix, "1", str(n)], capture_output=True, text=True)
+        r = subprocess.run([ORACLE_DUMP, "dump", mode, src, prefix, str(level), str(n)], capture_output=True, text=True)
         assert r.returncode == 0, "oracle_dump over %s:\n%s" % (name, (r.stdout + r.stderr)[-2000:])
         return Dump(prefix)
     # a reference process holds about 6 GB of models: four at a time, the longest streams first
     with ThreadPoolExecutor(min(len(names), 4)) as ex:
         futs = {name: ex.submit(dump, name) for name in sorted(names, key=lambda x: -inputs[x][2])}
         return {name: futs[name].result() for name in names}
+
+
+SMALL_COLS = list(range(3)) + list(range(2025, 2078))   # layer-0 inputs of the small models, PPMD and the LSTM
+
+
+def port_bit_for_bit(port, what, vocab, stream, ext, ppmd, p, small_inputs, inputs_first64, mix, ctx, lstm):
+    """The CPU port fed the reference's codes (ext [bits][2022]) and PPMD rows ([bytes][256]) over `stream`, against the
+    reference at every bit: Predict(), the 56 small-model and LSTM inputs (small_inputs [bits][56], SMALL_COLS of the
+    2078), all 2078 inputs on the first 64 bits, the 47 mixer outputs and the selectors; and the LSTM's 256-float
+    distribution after every byte. Fails with the first difference."""
+    vocab = np.ascontiguousarray(vocab, dtype=np.uint8)
+    P = port.op_create(vocab.ctypes.data)
+    bits = np.unpackbits(stream)
+    inp = np.zeros(2078, np.float32); out = np.zeros(47, np.float32); sel = np.zeros(47, np.uint32); lp = np.zeros(256, np.float32)
+    try:
+        for t in range(bits.size):
+            e = np.ascontiguousarray(ext[t])
+            got = port.op_predict(P, e.ctypes.data)
+            port.op_get_inputs(P, inp.ctypes.data)
+            port.op_get_mixer_outputs(P, out.ctypes.data)
+            port.op_get_mixer_contexts(P, sel.ctypes.data)
+            bad = [name for name, ok in (
+                ("Predict() (%.9g vs %.9g)" % (got, p[t]), np.float32(got) == p[t]),
+                ("small-model / LSTM inputs", np.array_equal(inp[SMALL_COLS], small_inputs[t])),
+                ("layer-0 inputs", t >= 64 or np.array_equal(inp, inputs_first64[t])),
+                ("mixer outputs", np.array_equal(out, mix[t])),
+                ("mixer selectors", np.array_equal(sel, ctx[t]))) if not ok]
+            if bad:
+                pytest.fail("%s: port differs from the reference at bit %d (byte %d): %s" % (what, t, t // 8, ", ".join(bad)),
+                            pytrace=False)
+            pp = np.ascontiguousarray(ppmd[t // 8])
+            port.op_perceive(P, int(bits[t]), pp.ctypes.data)
+            if t % 8 == 7:
+                port.op_get_lstm_probs(P, lp.ctypes.data)
+                if not np.array_equal(lp, lstm[t // 8]):
+                    pytest.fail("%s: port's LSTM byte distribution differs from the reference's after byte %d"
+                                % (what, t // 8), pytrace=False)
+    finally:
+        port.op_destroy(P)
 
 
 # ------------------------------------------------------------------------------------------------ child interpreters

@@ -8,33 +8,13 @@ import numpy as np
 import pytest
 
 from conftest import ROOT, port_replay, synthetic_streams
+from harness import port_bit_for_bit
 
 
-def test_port_matches_reference_bit_for_bit(port, golden):
+def test_port_matches_reference_bit_for_bit(port, golden, request):
     g = golden
-    vocab = np.ascontiguousarray(g.vocab)
-    P = port.op_create(vocab.ctypes.data)
-    bits = g.bits()
-    inp = np.zeros(2078, np.float32); mix = np.zeros(47, np.float32); ctx = np.zeros(47, np.uint32); lp = np.zeros(256, np.float32)
-    cols = list(range(3)) + list(range(2025, 2078))
-    for t in range(bits.size):
-        e = np.ascontiguousarray(g.ext[t])
-        p = port.op_predict(P, e.ctypes.data)
-        port.op_get_inputs(P, inp.ctypes.data)
-        port.op_get_mixer_outputs(P, mix.ctypes.data)
-        port.op_get_mixer_contexts(P, ctx.ctypes.data)
-        assert np.float32(p) == g.p[t], "Predict() differs at bit %d" % t
-        assert np.array_equal(inp[cols], g.small_inputs[t]), "small-model inputs differ at bit %d" % t
-        if t < 64:
-            assert np.array_equal(inp, g.inputs_first64[t])
-        assert np.array_equal(mix, g.mix[t]), "mixer outputs differ at bit %d" % t
-        assert np.array_equal(ctx, g.ctx[t]), "mixer selectors differ at bit %d" % t
-        pp = np.ascontiguousarray(g.ppmd[t // 8])
-        port.op_perceive(P, int(bits[t]), pp.ctypes.data)
-        if t % 8 == 7:
-            port.op_get_lstm_probs(P, lp.ctypes.data)
-            assert np.array_equal(lp, g.lstm[t // 8]), "LSTM byte distribution differs after byte %d" % (t // 8)
-    port.op_destroy(P)
+    port_bit_for_bit(port, request.node.callspec.params["golden"], g.vocab, g.stream, g.ext, g.ppmd, g.p, g.small_inputs,
+                     g.inputs_first64, g.mix, g.ctx, g.lstm)
 
 
 def _encode(port, p, bits):

@@ -28,14 +28,22 @@ from oracle_io import Dump  # noqa: E402
 ORACLE = os.path.join(ROOT, "oracle", "_ref", "oracle_dump")
 
 
-def make(name, tmp, gen=gen_stress, kind="stress"):
-    """tests/golden/<kind>_<name>.npz from stream `name` of generator module `gen` (gen_stress or gen_reach)."""
+def make(name, tmp, gen=gen_stress, kind="stress", dump=None):
+    """tests/golden/<kind>_<name>.npz from stream `name` of generator module `gen` (gen_stress, gen_reach or gen_vocab).
+    dump: the coded bytes the fixture keeps, when not the stream's length; the fixture then also holds `file_bytes`, the
+    length of the whole coded stream (whose byte set is the reference's vocabulary)."""
     n, seed = gen.STREAMS[name]
     src, prefix = os.path.join(tmp, name + ".bin"), os.path.join(tmp, name)
     gen.generate(name, n, seed).tofile(src)
+    extra = {}
+    if dump is not None:
+        n = dump
     subprocess.run([ORACLE, "dump", "n", src, prefix, "1", str(n)], check=True)
     d = Dump(prefix)
-    assert d.n_bytes == n and n % 512 == 0 and np.array_equal(d.stream, gen.coded_stream(name))
+    if dump is not None:
+        extra["file_bytes"] = np.array([int(d.meta["stream_bytes"])])
+    whole = n == int(d.meta["stream_bytes"])         # a whole stream may end inside a CRC block
+    assert d.n_bytes == n and (n % 512 == 0 or whole) and np.array_equal(d.stream, gen.coded_stream(name)[:n])
     nb = n * 8
     ext = d.ext
     crc_fx = np.array([zlib.crc32(np.ascontiguousarray(ext[b:b + 4096, :431]).tobytes()) for b in range(0, nb, 4096)], dtype=np.uint32)
@@ -45,7 +53,7 @@ def make(name, tmp, gen=gen_stress, kind="stress"):
     assert lstmfx.size == nb
     out = os.path.join(ROOT, "tests", "golden", "%s_%s.npz" % (kind, name))
     np.savez_compressed(out, stream=d.stream, vocab=d.vocab, p=d.p, crc_fx=crc_fx, crc_p8=crc_p8, first_codes=np.ascontiguousarray(ext[:64]),
-                        lstmfx=lstmfx, ppmd_crc=ppmd_crc, mode=np.array([d.meta["mode"]]), dictionary=np.array([0]))
+                        lstmfx=lstmfx, ppmd_crc=ppmd_crc, mode=np.array([d.meta["mode"]]), dictionary=np.array([0]), **extra)
     bits = np.unpackbits(d.stream)
     bpb = -np.log2(np.where(bits == 1, d.p, 1 - d.p).astype(np.float64)).sum() / n
     return "%-8s %5d bytes  %.3f bits/byte -> %d KiB" % (name, n, bpb, os.path.getsize(out) // 1024)
