@@ -114,6 +114,7 @@ struct P8Slot {
   int n2, nx, ncxt, base;
   int c0, bpos, blpos, st_type; u32 c4, st_match_length;
   u8 c1, st_match_expected, st_text_first, st_text_mask;
+  u8 relayout;                       // the set count differs from the previous bit's (ordinary <-> audio mode): p8_relayout
 };
 
 // Each 7-slot map lane's copy of the 7 state bytes of its slot (t[cp0 ..]) and the 2 bytes of its run record (t[runp ..]):
@@ -152,7 +153,9 @@ struct P8Shared {
     struct {                                                    // the model CTA
       unsigned long long seen[P8_SEEN];   // open-addressing set of (map, bucket) pairs touched this bit
       struct { double ch[3][32 * 33]; double pb[3][32]; } ols;   // Cholesky factor rows (padded) and a product buffer; byte boundaries only
+                                                                 // (in audio mode `ch` holds two vectors per audio OLS warp)
       P8CmCache cc;
+      int ncxt_handed;                    // the selector count of the last bit handed over (P8Slot::relayout)
 #ifdef P8_PROF
       long long leg_t[P8_CM_LANES];      // P8_LEG: when a lane's current leg started
 #endif
@@ -206,7 +209,11 @@ __constant__ signed char c_p8_unit_kind[P8_N_UNITS] = {
     1, 1, 1, -20, 1, 1, 1, 17, 11, -1, -2, 2, 2, 2, 2, 2, 2, 2, -3, 3, -4, -5, -6, -7, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2,
     -8, -9, -10, -11, -12, -13, -14, -15, 6, -16, -21, -22, 2, 2, 2, 2, 2};
 
-__device__ __forceinline__ int p8_unit_count(p8::State& S, int u, bool byte_start) {
+// In audio mode (paq8_top.h audio8_mode) the inputs are those of units 0-7, audio8bModel's 33 stationary maps in the place of
+// unit 8 and the record model's units 20-35; the other units add nothing.
+__device__ __forceinline__ int p8_unit_count(p8::State& S, int u, bool byte_start, bool audio) {
+  if (audio && u == 8) return 2 * p8::AUDIO_N_SCM;
+  if (audio && ((u > 8 && u < 20) || u > 35)) return 0;
   const int kind = c_p8_unit_kind[u];
   if (kind >= 0) return kind;
   if (kind <= -20) { const int k = -20 - kind; return 7 * (byte_start ? (int)c_p8_cm2_cap[k] : p8_cm2(S, k).index); }
@@ -214,7 +221,25 @@ __device__ __forceinline__ int p8_unit_count(p8::State& S, int u, bool byte_star
   return 5 * (byte_start ? (int)c_p8_cm_full[k] : p8_cm(S, k).cn);
 }
 
+// unit_off[]: the mixer-input offset of every unit (one warp, prefix sums)
+__device__ __noinline__ void p8_unit_offsets(P8Shared& sh, int lane, bool byte_start, bool audio) {
+  const unsigned full = 0xffffffffu;
+  const int a = p8_unit_count(sh.S, lane, byte_start, audio);
+  const int b = lane + 32 < P8_N_UNITS ? p8_unit_count(sh.S, lane + 32, byte_start, audio) : 0;
+  int ia = a, ib = b;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int va = __shfl_up_sync(full, ia, d), vb = __shfl_up_sync(full, ib, d);
+    if (lane >= d) { ia += va; ib += vb; }
+  }
+  const int ta = __shfl_sync(full, ia, 31);
+  sh.unit_off[lane] = ia - a;
+  if (lane + 32 <= P8_N_UNITS) sh.unit_off[lane + 32] = ta + ib - b;
+}
+
 __device__ __forceinline__ p8::Out p8_out(P8Shared& sh, int offset) { p8::Out o; o.T = sh.S.T; o.tx = sh.S.m.tx; o.codes = sh.S.codes; o.n = offset; return o; }
+// audio8bModel's stationary map q, its inputs in the place of unit 8 (p8_unit_count)
+__device__ __noinline__ void p8_audio_scm(P8Shared& sh, int q) { p8::Out o = p8_out(sh, sh.unit_off[8] + 2 * q); p8::audio8b_scm(sh.S, o, q); }
 
 __device__ __forceinline__ void p8_copy_words(void* dst, const void* src, size_t bytes, int tid) {
   u32* d = (u32*)dst; const u32* s = (const u32*)src;
@@ -307,6 +332,89 @@ __device__ __noinline__ void p8_ols_byte_warp(P8Shared& sh, int k, int lane) {
     for (int i = 0; i < 32; ++i) sum = P8_DADD(sum, pb[i]);
     M.prd[k] = (u8)clip8((int)P8_FLOOR(sum));
     M.ols_km[k] = km;
+  }
+  __syncwarp();
+}
+
+// One OLS predictor k of audio8bModel at a byte boundary, on one warp (paq8_top.h audio8b_ols): OLS::Update(s) on channel
+// pCh, then the taps and Predict() on channel ch. Element-wise steps use any lane mapping; every SUM runs in the reference's
+// order. Rows go to lanes round robin; sums and products of a step meet in two shared-memory vectors of the warp (u, v):
+//  * covariance and b: lane = column (the matrix stays exactly symmetric);
+//  * Factor() column by column, the rows of a column side by side, each inner sum over k < c in ascending order. The factor
+//    is kept TRANSPOSED in the block's chol[][] (column c contiguous, so a step reads consecutive doubles); a failed
+//    diagonal stops it as the reference's row order does (w is kept);
+//  * forward substitution column by column (row i subtracts in ascending j), backward substitution row by row with the
+//    products gathered and summed in ascending order; Predict() sums on lane 0.
+// Kept small on purpose: it runs once per sample, and its code shares the instruction cache with the ordinary bits.
+__device__ __noinline__ void p8_audio_ols_warp(P8Shared& sh, int k, int lane) {
+  using namespace p8;
+  State& S = sh.S;
+  AudioM& A = *S.audio;
+  const int n = audio_ols_n(k), pch = A.ch ^ A.stereo;
+  const double lambda = audio_ols_lambda(k), nu = 0.001, one_minus = P8_DSUB(1.0, lambda);
+  double* blk = audio_ols_block(A, k, pch);
+  double* x = blk; double* w = blk + n; double* b = blk + 2 * n; double* cov = blk + 3 * n; double* lt = cov + n * n;
+  double* u = sh.u.md.ols.ch[0] + (k == 7 ? 6 : k) * 256; double* v = u + 128;
+  const double val = (double)(buf(S, 1) - 128);
+  int km = A.ols_km[k][pch] + 1;
+  const bool solve = km >= audio_ols_kmax(k);
+  for (int j = 0; j < n; ++j) {
+    const double xj = x[j];
+    for (int i = lane; i < n; i += 32) {
+      const double c = P8_DADD(P8_DMUL(lambda, cov[j * n + i]), P8_DMUL(one_minus, P8_DMUL(xj, x[i])));
+      cov[j * n + i] = c;
+      if (solve) lt[j * n + i] = i == j ? P8_DADD(c, nu) : c;     // column j of the copy is row j: the matrix is symmetric
+    }
+  }
+  for (int i = lane; i < n; i += 32) { b[i] = P8_DADD(P8_DMUL(lambda, b[i]), P8_DMUL(one_minus, P8_DMUL(x[i], val))); v[i] = b[i]; }
+  if (solve) {
+    __syncwarp();
+    bool fail = false;
+    for (int c = 0; c < n && !fail; ++c) {
+      for (int r = c + lane; r < n; r += 32) {
+        double s = lt[c * n + r];
+        for (int q = 0; q < c; ++q) s = P8_DSUB(s, P8_DMUL(lt[q * n + r], lt[q * n + c]));
+        u[r] = s;
+      }
+      __syncwarp();
+      const double d = u[c];
+      if (d > 1E-8) {
+        const double dd = P8_DSQRT(d);
+        for (int r = c + lane; r < n; r += 32) lt[c * n + r] = r == c ? dd : P8_DDIV(u[r], dd);
+      } else fail = true;
+      __syncwarp();
+    }
+    if (!fail) {
+      for (int q = 0; q < n; ++q) {            // v: the rows' running sums; u: w after the forward pass
+        const double wq = P8_DDIV(v[q], lt[q * n + q]);
+        for (int r = q + 1 + lane; r < n; r += 32) v[r] = P8_DSUB(v[r], P8_DMUL(lt[q * n + r], wq));
+        if (lane == 0) u[q] = wq;
+        __syncwarp();
+      }
+      for (int i = n - 1; i >= 0; --i) {       // v: the products of row i; u[i]: w[i] after the backward pass
+        for (int j = i + 1 + lane; j < n; j += 32) v[j] = P8_DMUL(lt[i * n + j], u[j]);
+        __syncwarp();
+        if (lane == 0) {
+          double s = u[i];
+          for (int j = i + 1; j < n; ++j) s = P8_DSUB(s, v[j]);
+          u[i] = P8_DDIV(s, lt[i * n + i]);
+        }
+        __syncwarp();
+      }
+      for (int i = lane; i < n; i += 32) w[i] = u[i];
+    }
+    km = 0;
+  }
+  __syncwarp();
+  if (lane == 0) { A.ols_km[k][pch] = km; audio8b_taps(S, k); }
+  __syncwarp();
+  const double* xc = audio_ols_block(A, k, A.ch);
+  for (int i = lane; i < n; i += 32) v[i] = P8_DMUL(xc[n + i], xc[i]);
+  __syncwarp();
+  if (lane == 0) {
+    double sum = 0.;
+    for (int i = 0; i < n; ++i) sum = P8_DADD(sum, v[i]);
+    audio8b_predict(S, k, sum);
   }
   __syncwarp();
 }
@@ -443,10 +551,11 @@ __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, i
 }
 // the units that are one lane each, on the bit that starts a byte (warps 8-11 of the D-chain; record_pre and the linear
 // predictions' maps follow their models there)
-__device__ __noinline__ void p8_probe_single(P8Shared& sh, int tid, int y, int c0, int bpos) {
+__device__ __noinline__ void p8_probe_single(P8Shared& sh, int tid, int y, int c0, int bpos, bool audio) {
   using namespace p8;
   State& S = sh.S;
   const p8::Tables& T = *S.T;
+  if (audio && (tid == P8_TID_PIC || (tid >= P8_TID_W10 && tid < P8_TID_W10 + 10) || tid == P8_TID_W11)) return;   // not in audio mode
   if (tid == P8_TID_PIC) pic_core(S);
   else if (tid == P8_TID_MATCH) { Out o = p8_out(sh, sh.unit_off[7]); match_core(S, o); }
   else if (tid >= P8_TID_W10 && tid < P8_TID_W10 + 10) sh.dmc_st[tid - P8_TID_W10] = dmc_st(T, S.dmc[tid - P8_TID_W10], y);
@@ -554,9 +663,10 @@ __device__ __forceinline__ void p8_dmc_mix(P8Shared& sh, p8::Out& o, int bpos) {
       if ((S.dmc[i].extra >> 7) > S.dmc[i].size) dmc_reset(S.dmc[i], params[i]);
 }
 // the units that are one lane each, on the bit that starts a byte (warps 9-11 after the join)
-__device__ __noinline__ void p8_apply_small(P8Shared& sh, int tid, int y, int bpos) {
+__device__ __noinline__ void p8_apply_small(P8Shared& sh, int tid, int y, int bpos, bool audio) {
   using namespace p8;
   State& S = sh.S;
+  if (audio && tid >= P8_TID_W10 + 12) return;   // audio mode: the match and record models' maps only
   if (tid >= P8_TID_MATCH && tid < P8_TID_MATCH + 9) {   // the nine maps behind the match model
     Out o = p8_out(sh, sh.unit_off[7]);
     match_unit(S, o, tid - P8_TID_MATCH);
@@ -580,10 +690,17 @@ __device__ __noinline__ void p8_apply_small(P8Shared& sh, int tid, int y, int bp
 
 // ---- inside a byte: the single-lane units, a warp per function (lane map: P8_W_* below). Every unit writes its inputs at
 // its own unit_off[] as on the bit that starts a byte; units of one phase share no state, so their order does not matter.
-__device__ __noinline__ void p8_probe_units(P8Shared& sh, int warp, int lane, int y, int c0, int bpos) {
+// In audio mode the DMC, sparse match and picture units do not run; warps 10 and 11 run audio8bModel's 33 maps instead.
+__device__ __noinline__ void p8_probe_units(P8Shared& sh, int warp, int lane, int y, int c0, int bpos, bool audio) {
   using namespace p8;
   State& S = sh.S;
   P8_U0;
+  if (audio && (warp == P8_W_DMC || warp == P8_W_SMATCH)) {
+    const int q = warp == P8_W_DMC ? lane : 32 + lane;
+    if (q < AUDIO_N_SCM) p8_audio_scm(sh, q);
+    return;
+  }
+  if (audio && warp == P8_W_PIC) return;
   if (warp == P8_W_MATCH) {
     if (lane == 0) { Out o = p8_out(sh, sh.unit_off[7]); match_core(S, o); P8_U(1); }
   } else if (warp == P8_W_DMC) {
@@ -600,11 +717,13 @@ __device__ __noinline__ void p8_probe_units(P8Shared& sh, int warp, int lane, in
 }
 // The apply phase groups the units by the map they end in, so that the lanes of a warp run one call of one function with
 // their own arguments (the arguments are those of match_unit, record_small, smatch_unit, linear_small and the rest).
-__device__ __noinline__ void p8_apply_units(P8Shared& sh, int warp, int lane, int y, int c0, int bpos) {
+__device__ __noinline__ void p8_apply_units(P8Shared& sh, int warp, int lane, int y, int c0, int bpos, bool audio) {
   using namespace p8;
   State& S = sh.S;
   const p8::Tables& T = *S.T;
   P8_U0;
+  // audio mode: the maps behind the match and record models and the constant input only
+  if (audio && ((warp == P8_W_SCM && lane >= 6) || (warp == P8_W_STM && lane >= 9) || warp == P8_W_PICU || (warp == P8_W_DMCMIX && lane == 0))) return;
   if (warp == P8_W_SM32) {              // the match model's three StateMaps (match_unit 0-2), the order-0 and order-1 inputs
     if (lane >= 5) return;
     Sm32* s; int off, cx; bool on = true;
@@ -750,6 +869,33 @@ static_assert(P8_W_MATCH > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_SM
               P8_W_IMAP > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_DMCMIX < (int)P8_MAP_WARPS && (int)P8_W_SM32 == (int)P8_WARP_TEXT && (int)P8_W_STM == (int)P8_WARPS - 1,
               "barrier 3 inside a byte: the unit warps are 9-11 (in barriers 1 and 2 with the map warps) and 13-15 (in barrier 3 only)");
 
+// The mixer CTA's first bit in a new layout, on one warp: every cached row back to HBM, then the bit's sets fetched and their
+// dot products (no row is fetched before every row is written back, and no other warp reads them this bit)
+__device__ __noinline__ void p8_relayout(P8Shared& sh, const P8Slot& in, int lane) {
+  using namespace p8;
+  const Mixer& m = sh.S.m;
+  for (int i = 0; i < N_SETS; ++i) if (sh.wc_set[i] >= 0) p8_row_store(m.w + (size_t)sh.wc_set[i] * N_IN, sh.u.mx.wc[i], lane);
+  __syncwarp();
+  if (lane < N_SETS) sh.wc_set[lane] = -1;
+  for (int i = 0; i < in.ncxt; ++i) {
+    short* row = sh.u.mx.wc[i];
+    p8_row_load(row, m.w + (size_t)m.cxt[i] * N_IN, lane);
+    __syncwarp();
+    if (lane == 0) sh.wc_set[i] = m.cxt[i];
+    int acc = 0;
+    for (int q = lane; q < (in.nx >> 3); q += 32) {
+      const uint4 wv = *reinterpret_cast<const uint4*>(row + q * 8);
+      const uint4 xv = *reinterpret_cast<const uint4*>(in.tx + q * 8);
+      const short* w = reinterpret_cast<const short*>(&wv);
+      const short* x = reinterpret_cast<const short*>(&xv);
+#pragma unroll
+      for (int e = 0; e < 8; e += 2) acc += dot_pair(x + e, w + e);
+    }
+    acc = __reduce_add_sync(0xffffffffu, acc);
+    if (lane == 0) sh.dot[i] = acc;
+  }
+}
+
 // Mixer::update for the 28 cached weight sets selected for the previous bit, on its inputs tx (all lanes of the mixer CTA)
 __device__ __forceinline__ void p8_sgd(P8Shared& sh, const short* tx, int y, int tid) {
   using namespace p8;
@@ -774,6 +920,8 @@ __device__ __forceinline__ void p8_sgd(P8Shared& sh, const short* tx, int y, int
   }
 }
 
+__device__ __noinline__ void p8_audio_selects(p8::State& S) { p8::audio8b_select(S); p8::record_select(S); }
+
 // The model CTA's part of bit t of a launch: PAQ8::Perceive(y) up to the mixer's inputs and selectors, handed to slot t % P8_RING
 // of the mixer CTA's ring (`ring`: that array in the mixer CTA). All P8_THREADS lanes call it: warps 0-11 evaluate the models,
 // warp 12 computes ModelStats and 19 selector sets beside them.
@@ -791,6 +939,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     P8_U0;
     bit_begin(S, y);
     if (S.bpos == 0) block_parse(S);
+    if (S.bpos == 0 && audio8_mode(S)) audio8b_begin(S);
     P8_U(20);
     if (S.bpos == 0) sh.snap = word_stats(S);     // read by sparse1_byte only
     P8_U(21);
@@ -799,21 +948,12 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
   if (tid >= 64 && tid < 64 + P8_N_CM2) { sh.clash2[tid - 64] = 0; sh.res2[tid - 64] = 0; }
   if (tid == 67) sh.any_clash = 0;
   if (warp == 11) p8_draw_seq(sh, lane);          // beside lane 0's bit_begin: the draws depend on the generator only
-  if (tid >= P8_CM2_TID0 && tid < P8_CM2_TID0 + P8_N_CM2) cm2_begin(p8_cm2(S, tid - P8_CM2_TID0), y, nb);
-  if (warp == P8_WARPS - 1 && (nb <= 1 || fresh)) {      // mixer-input offsets of the units (they change on the first two bits of a byte only)
-    const unsigned full = 0xffffffffu;
-    const int a = p8_unit_count(S, lane, nb == 0);
-    const int b = lane + 32 < P8_N_UNITS ? p8_unit_count(S, lane + 32, nb == 0) : 0;
-    int ia = a, ib = b;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int va = __shfl_up_sync(full, ia, d), vb = __shfl_up_sync(full, ib, d);
-      if (lane >= d) { ia += va; ib += vb; }
-    }
-    const int ta = __shfl_sync(full, ia, 31);
-    sh.unit_off[lane] = ia - a;
-    if (lane + 32 <= P8_N_UNITS) sh.unit_off[lane + 32] = ta + ib - b;
-  }
+  // the history maps' bit prologue; the text and x86 maps do not run in audio mode, so on the bit that starts a byte theirs
+  // waits until lane 0 has parsed the byte (D-chain)
+  if (tid >= P8_CM2_TID0 && tid < P8_CM2_TID0 + P8_N_CM2 && (tid == P8_CM2_TID0 || (nb != 0 && !audio8_mode(S)))) cm2_begin(p8_cm2(S, tid - P8_CM2_TID0), y, nb);
+  // mixer-input offsets of the units (they change on the first two bits of a byte only). Audio mode is known here inside a
+  // byte; on the bit that starts one lane 0 is deciding it, and warp 11 redoes the offsets of an audio byte after the barrier
+  if (warp == P8_WARPS - 1 && (nb <= 1 || fresh)) p8_unit_offsets(sh, lane, nb == 0, nb != 0 && audio8_mode(S));
   {
     P8_U0;
     for (int k = tid; k < P8_SEEN; k += P8_THREADS) sh.u.md.seen[k] = 0ull;
@@ -823,10 +963,12 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
   P8_T(0);
   const int bpos = S.bpos, c0 = S.c0;
   const bool byte_start = bpos == 0;
+  const bool audio = audio8_mode(S);      // audioModel's bits: audio8bModel and recordModel(AUDIO) behind the shared prefix
   if (tid >= P8_MAP_THREADS) {
     if (warp == P8_MAP_WARPS) {            // ModelStats and the 19 selector sets that do not wait for the order-N map
       p8_await_selects(JIT_HERE);
-      if (lane == 0) {
+      if (lane == 0 && audio) p8_audio_selects(S);   // audio mode: its own 8 sets from weight set 0
+      else if (lane == 0) {
         xml_stats(S);
         smatch_select(S);
         record_select(S);
@@ -837,40 +979,43 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       }
     } else if (byte_start) {
       // ---- byte boundary, the text chain (warps 13-15): state on one lane, the three stemmers of a completed word a warp
-      // each, then the 33 contexts side by side. Nothing else reads the text model before the join.
+      // each, then the 33 contexts side by side. Nothing else reads the text model before the join (in audio mode it does
+      // not run: the three warps go straight to the join)
       P8_M0;
-      if (tid == P8_WARP_TEXT * 32) sh.text_pending = text_update_a(S);
-      p8_sync_text(JIT_HERE);
-      if (sh.text_pending) {
-        const int split = S.text.stem_split;
-        const int i = warp == P8_WARP_TEXT ? LANG_EN : (warp == P8_WARP_TEXT + 1 ? LANG_FR : LANG_DE);
-        if (lane == 0 && i >= split) text_stem(S, i);
+      if (!audio) {
+        if (tid == P8_WARP_TEXT * 32) sh.text_pending = text_update_a(S);
         p8_sync_text(JIT_HERE);
-        if (tid == P8_WARP_TEXT * 32) {
-          text_stem_mid(S);
-          for (int j = split - 1; j > LANG_UNKNOWN; --j) text_stem(S, j);
-          text_update_b(S);
+        if (sh.text_pending) {
+          const int split = S.text.stem_split;
+          const int i = warp == P8_WARP_TEXT ? LANG_EN : (warp == P8_WARP_TEXT + 1 ? LANG_FR : LANG_DE);
+          if (lane == 0 && i >= split) text_stem(S, i);
+          p8_sync_text(JIT_HERE);
+          if (tid == P8_WARP_TEXT * 32) {
+            text_stem_mid(S);
+            for (int j = split - 1; j > LANG_UNKNOWN; --j) text_stem(S, j);
+            text_update_b(S);
+          }
         }
-      }
-      if (warp == P8_WARP_TEXT) {
-        __syncwarp();
-        const int n = text_contexts(S, CtxSel{lane, 32});
-        __syncwarp();
-        if (lane == 0) { S.text.map.index = n; P8_M(38); }
+        if (warp == P8_WARP_TEXT) {
+          __syncwarp();
+          const int n = text_contexts(S, CtxSel{lane, 32});
+          __syncwarp();
+          if (lane == 0) { S.text.map.index = n; P8_M(38); }
+        }
       }
       p8_join_arrive(JIT_HERE);
     } else {
       // ---- inside a byte, warps 13-15: single-lane units beside the maps; the apply runs while lane 0 numbers a clashing bit
       {
         P8_M0;
-        p8_probe_units(sh, warp, lane, y, c0, bpos);
+        p8_probe_units(sh, warp, lane, y, c0, bpos, audio);
         __syncwarp();
         if (lane == 0) P8_M(24 + warp);
       }
       p8_join_sync(JIT_HERE);
       {
         P8_M0;
-        p8_apply_units(sh, warp, lane, y, c0, bpos);
+        p8_apply_units(sh, warp, lane, y, c0, bpos, audio);
         __syncwarp();
         if (lane == 0) P8_M(48 + warp);
       }
@@ -884,21 +1029,27 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         if (warp >= P8_WARP_D) {
           // the D-chain: order-N and x86 contexts -> their history maps and the single-lane units -> the sparse and record
           // models, which consume the order-N map's result and the match length of this bit
+          // (in audio mode the order-N map, the match model and the record model only)
+          if (audio && warp == P8_MAP_WARPS - 1) p8_unit_offsets(sh, lane, true, true);
           if (tid == P8_CM2_TID0) ordern_byte(S);
-          else if (tid == P8_TID_MATCH) exe_byte(S);
+          else if (tid == P8_TID_MATCH && !audio) exe_byte(S);
+          else if ((tid == P8_CM2_TID0 + 1 || tid == P8_CM2_TID0 + 2) && !audio) cm2_begin(p8_cm2(S, tid - P8_CM2_TID0), y, 0);
           p8_sync_dchain(JIT_HERE);
           if (tid == P8_CM2_TID0) P8_M(31);
-          p8_probe_cm2(sh, tid, bpos, 5);
-          p8_probe_single(sh, tid, y, c0, bpos);
+          p8_probe_cm2(sh, tid, bpos, audio ? 1 : 5);
+          p8_probe_single(sh, tid, y, c0, bpos, audio);
           p8_sync_dchain(JIT_HERE);
           if (tid == P8_CM2_TID0) P8_M(32);
-          p8_apply_cm2(sh, tid, y, bpos, 5);
+          p8_apply_cm2(sh, tid, y, bpos, audio ? 1 : 5);
           p8_sync_dchain(JIT_HERE);
           if (tid == P8_CM2_TID0) P8_M(33);
           const int ismatch = ilog(T, S.match.length);
-          if (tid == P8_TID_MATCH) { sparse_byte(S, ismatch, sh.res2[0]); P8_M(34); }
-          else if (tid == P8_TID_W10) { sparse1_byte(S, ismatch, sh.res2[0], sh.snap); P8_M(35); }
-          else if (tid == P8_TID_W11) { record_byte(S); record_pre(S); P8_M(36); }
+          if (tid == P8_TID_MATCH && !audio) { sparse_byte(S, ismatch, sh.res2[0]); P8_M(34); }
+          else if (tid == P8_TID_W10 && !audio) { sparse1_byte(S, ismatch, sh.res2[0], sh.snap); P8_M(35); }
+          else if (tid == P8_TID_W11) { record_byte(S, audio ? FT_AUDIO : S.filetype); record_pre(S); P8_M(36); }
+        } else if (audio) {         // audio mode: the eight OLS predictors of the channel, a warp each (OLS 6 and 7 share warp 6)
+          p8_audio_ols_warp(sh, warp, lane);
+          if (warp == 6) p8_audio_ols_warp(sh, 7, lane);
         } else if (warp < 3) {      // a linear predictor per warp, then the map behind it
           p8_ols_byte_warp(sh, warp, lane);
           if (lane == 0) { Out o = p8_out(sh, sh.unit_off[48 + warp]); linear_small(S, o, warp); }
@@ -935,7 +1086,8 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       P8_T(7);
       p8_apply_cm(sh, tid, y, c0, bpos);
       p8_apply_cm2(sh, tid, y, bpos, 2);
-      p8_apply_small(sh, tid, y, bpos);
+      p8_apply_small(sh, tid, y, bpos, audio);
+      if (audio && tid >= P8_CM2_TID0 && tid < P8_CM2_TID0 + AUDIO_N_SCM) p8_audio_scm(sh, tid - P8_CM2_TID0);   // behind the predictions
       p8_sync_maps(JIT_HERE);
       P8_T(8);
     } else {
@@ -945,7 +1097,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         P8_M0;
         if (warp < 7) p8_probe_cm(sh, tid, y, c0, bpos);
         else if (warp < P8_W_MATCH) p8_probe_cm2(sh, tid, bpos, 7);
-        else p8_probe_units(sh, warp, lane, y, c0, bpos);
+        else p8_probe_units(sh, warp, lane, y, c0, bpos, audio);
         __syncwarp();
         if (lane == 0) P8_M(24 + warp);
       }
@@ -958,7 +1110,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         P8_M0;
         if (warp < 7) p8_apply_cm(sh, tid, y, c0, bpos);
         else if (warp < P8_W_IMAP) p8_apply_cm2(sh, tid, y, bpos, 7);
-        else p8_apply_units(sh, warp, lane, y, c0, bpos);
+        else p8_apply_units(sh, warp, lane, y, c0, bpos, audio);
         __syncwarp();
         if (lane == 0) P8_M(48 + warp);
       }
@@ -972,7 +1124,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         for (int k = 0; k < P8_N_CM; ++k) if (!sh.clash[k]) p8_cm(S, k).cn = 0;
         for (int k = 0; k < P8_N_CM2; ++k) p8_cm2(S, k).index = 0;
       }
-      main_select_fixed(S, sh.res2[0]);      // sets 19..27; warp 12 writes 0..18 (and the count) beside this
+      if (!audio) main_select_fixed(S, sh.res2[0]);      // sets 19..27; warp 12 writes 0..18 (and the count) beside this
       Mixer& m = S.m;
       m.nx = sh.unit_off[P8_N_UNITS];
       m.n2 = m.nx;
@@ -1000,6 +1152,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
         d.n2 = m.n2; d.nx = m.nx; d.ncxt = m.ncxt; d.base = m.base;
         d.c0 = S.c0; d.bpos = S.bpos; d.blpos = S.blpos; d.st_type = S.st_type; d.c4 = S.c4; d.st_match_length = S.st_match_length;
         d.c1 = (u8)buf(S, 1); d.st_match_expected = S.st_match_expected; d.st_text_first = S.st_text_first; d.st_text_mask = S.st_text_mask;
+        d.relayout = sh.u.md.ncxt_handed != m.ncxt; sh.u.md.ncxt_handed = m.ncxt;
       }
     }
     for (int q = tid; q < m.nx / 8; q += P8_THREADS) reinterpret_cast<uint4*>(d.tx)[q] = reinterpret_cast<const uint4*>(m.tx)[q];
@@ -1048,7 +1201,7 @@ __device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_p
   // ---- the bit's inputs and selectors (set 26 from this CTA's last prediction)
   mbar_wait(&sh.full[slot], (t / P8_RING) & 1, JIT_HERE);
   P8_T(16);
-  if (tid < N_SETS) m.cxt[tid] = tid == MAIN_SET_FIRST + 7 ? MAIN_SET_PR + S.last_prediction / 16 : in.cxt[tid];
+  if (tid < N_SETS) m.cxt[tid] = tid == MAIN_SET_FIRST + 7 && in.ncxt == N_SETS ? MAIN_SET_PR + S.last_prediction / 16 : in.cxt[tid];
   JIT_SYNCTHREADS();
   if (tid == 0) {
     if (t > 0) mbar_arrive_remote(&sh.empty[(t - 1) % P8_RING], 0, JIT_HERE);   // tx_prev was slot t-1's
@@ -1066,7 +1219,11 @@ __device__ void p8_mix_bit(P8Shared& sh, u32 t, int y, int nb, const short* tx_p
       for (int j = 0; j < lane; ++j) dup = dup || m.cxt[j] == m.cxt[lane];
       if (dup) S.error |= ERR_MIXER_ALIAS;
     }
-    for (int i = warp; i < in.ncxt; i += P8_WARPS) {
+    // A change of layout (ordinary <-> audio mode, 28 <-> 8 sets) gives the cached rows' selectors other meanings: a set still
+    // cached under one selector could be fetched fresh from HBM under another. Such a bit writes every row back first and
+    // fetches its sets on warp 0 alone.
+    if (in.relayout && warp == 0) p8_relayout(sh, in, lane);
+    for (int i = in.relayout ? N_SETS : warp; i < in.ncxt; i += P8_WARPS) {
       short* row = sh.u.mx.wc[i];
       const int set = m.cxt[i], old = sh.wc_set[i];
       if (old != set) {
@@ -1122,6 +1279,7 @@ __device__ __forceinline__ const p8::Tables* p8_enter(P8Shared& sh, p8::State* g
   p8_copy_words(sh.tab, gT, p8::TABLES_HOT_BYTES, tid);
   if (tid < p8::N_SETS) sh.wc_set[tid] = -1;
   if (rank == 0) for (int k = tid; k < P8_CM_LANES; k += P8_THREADS) sh.u.md.cc.valid[k] = 0;   // shared memory is new
+  if (rank == 0 && tid == 0) sh.u.md.ncxt_handed = sh.S.m.ncxt;
 #ifdef P8_PROF
   for (int k = tid; k < P8_PROF_SLOTS; k += P8_THREADS) sh.prof_acc[k] = 0;
 #endif

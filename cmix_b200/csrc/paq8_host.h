@@ -347,6 +347,15 @@ template <class B> bool build_state(B& be, const Tables& T, State& S) {
     for (int k = 0; k < 5; ++k) b.scm(M.smap[k], 11, 1);
     M.ols = b.template alloc<double>((size_t)3 * OLS_STRIDE);
   }
+  {
+    AudioM A;
+    memset(&A, 0, sizeof A);
+    for (int i = 0; i < AUDIO_N_PRD; ++i) for (int j = 0; j < 3; ++j) b.scm(A.scm[i][j], 11, 1);
+    A.ols = b.template alloc<double>((size_t)AUDIO_OLS_DOUBLES);
+    S.audio = b.template alloc<AudioM>(1);
+    if (!b.ok) return false;
+    be.upload(S.audio, &A, sizeof A);
+  }
   S.m.w = b.template alloc<short>((size_t)N_WSETS * N_IN);
   S.m.w2 = b.template alloc<short>(32);
   if (!b.ok) return false;

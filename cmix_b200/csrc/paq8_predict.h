@@ -94,6 +94,17 @@ struct DetectM {   // the header detectors in front of the image / audio / JPEG 
   u32 wav_header, wav_channels, wav_bits, wav_chunk;   // audioModel's WAVAudio (:5806-5808)
   u32 wav_length, wav_eoi, wav_info;                   // and its statics `length`, `eoi`, `info` (:5811)
 };
+// audio8bModel (:5552-5657): eight OLS<double, int8_t> predictors and three fixed ones per channel, three stationary maps
+// behind each predictor; `wmode` is the file-wide static X1 / X2 read (:5511). Lives in HBM (State::audio).
+enum { AUDIO_N_OLS = 8, AUDIO_N_PRD = 11, AUDIO_N_SCM = 3 * AUDIO_N_PRD };
+struct AudioM {
+  Scm scm[AUDIO_N_PRD][3];
+  double* ols;                   // the 16 OLS blocks (predictor k, channel c) at audio_ols_block
+  int ols_km[AUDIO_N_OLS][2], ols_index[AUDIO_N_OLS][2];
+  int prd[AUDIO_N_PRD][2][2], residuals[AUDIO_N_PRD][2];
+  int stereo, ch, rpos, last_pos, wmode;
+  u32 mask, err_log, mx_ctx;
+};
 
 struct State {
   const Tables* T;
@@ -118,6 +129,7 @@ struct State {
   // outputs
   u16 codes[N_OUT + 1];
   u32 error;
+  AudioM* audio;         // in HBM: the shared-memory copy of the state block keeps its size (the pointer fills its tail padding)
 };
 
 P8_HD inline int buf(const State& S, int i) { return S.buf[(u32)(S.pos - i) & P8_BUF_MASK]; }
@@ -422,7 +434,7 @@ P8_HD inline void pic_bit(State& S, Out& o) {
 }
 
 // ---------------------------------------------------------------- record models (:4204-4474)
-P8_COLD P8_HD inline void record_byte(State& S) {
+P8_COLD P8_HD inline void record_byte(State& S, int filetype) {   // filetype: recordModel's argument (FT_AUDIO in audio mode)
   const Tables& T = *S.T;
   RecordM& M = S.record;
   const u32 c4 = S.c4;
@@ -430,7 +442,7 @@ P8_COLD P8_HD inline void record_byte(State& S) {
   if (S.st_record && (S.st_record >> 16) != (u32)M.rlen[0]) { M.rlen[0] = (int)(S.st_record >> 16); M.rcount[0] = M.rcount[1] = 0; }
   else {
     if (blpos == 0 || (M.db_version > 0 && blpos >= M.db_end)) M.db_version = 0;
-    else if (M.db_version == 0 && (S.filetype == FT_DEFAULT || S.filetype == FT_TEXT) && blpos >= 31) {
+    else if (M.db_version == 0 && (filetype == FT_DEFAULT || filetype == FT_TEXT) && blpos >= 31) {
       u8 b = (u8)buf(S, 32);
       bool ok = ((b & 7) == 3 || (b & 7) == 4 || (b >> 4) == 3 || b == 0xF5);
       if (ok) { b = (u8)buf(S, 30); ok = b > 0 && b < 13; }
@@ -566,11 +578,11 @@ P8_HD inline void record_select(State& S) {   // selector sets and ModelStats (:
   mset(S.m, (S.grp0 << 5) | M.x, 11 * 32);
   S.st_record = ((u32)imin(0xFFFF, M.rlen[0]) << 16) | (u32)imin(0xFFFF, M.col);
 }
-P8_HD inline void record_core(State& S, Out& o, Rnd& rnd) {
+P8_HD inline void record_core(State& S, Out& o, Rnd& rnd, int filetype) {
   RecordM& M = S.record;
   const int y = S.y, bpos = S.bpos, c0 = S.c0;
   const int c1 = buf(S, 1);
-  if (bpos == 0) record_byte(S);
+  if (bpos == 0) record_byte(S, filetype);
   record_pre(S);
   cm_mix(M.cm, o, rnd, y, c0, bpos, c1);
   cm_mix(M.cn, o, rnd, y, c0, bpos, c1);

@@ -637,41 +637,49 @@ enum { OLS_N = 32, OLS_STRIDE = 3 * 32 + 2 * 32 * 32 };
 #define P8_DSQRT(a) sqrt(a)
 #define P8_FLOOR(a) floor(a)
 #endif
-P8_HD inline void ols_update(double* blk, int& km, u8 val) {
-  const double lambda = 0.995, nu = 0.001, one_minus = 1.0 - 0.995;
-  double* x = blk; double* w = blk + 32; double* b = blk + 64; double* cov = blk + 96; double* ch = blk + 96 + 1024;
-  for (int j = 0; j < OLS_N; ++j)
-    for (int i = 0; i < OLS_N; ++i) cov[j * 32 + i] = P8_DADD(P8_DMUL(lambda, cov[j * 32 + i]), P8_DMUL(one_minus, P8_DMUL(x[j], x[i])));
-  for (int i = 0; i < OLS_N; ++i) b[i] = P8_DADD(P8_DMUL(lambda, b[i]), P8_DMUL(one_minus, P8_DMUL(x[i], (double)val)));
+// OLS<double, T>::Update(val) (:1453-1464) on a block x[n], w[n], b[n], cov[n][n], chol[n][n]: hasZeroMean, so sub = 0,
+// nu = 0.001, ftol = 1e-8; a failed Factor() keeps w.
+P8_HD inline void ols_update(double* blk, int n, int kmax, double lambda, int& km, double val) {
+  const double nu = 0.001, one_minus = P8_DSUB(1.0, lambda);
+  double* x = blk; double* w = blk + n; double* b = blk + 2 * n; double* cov = blk + 3 * n; double* ch = cov + n * n;
+  for (int j = 0; j < n; ++j)
+    for (int i = 0; i < n; ++i) cov[j * n + i] = P8_DADD(P8_DMUL(lambda, cov[j * n + i]), P8_DMUL(one_minus, P8_DMUL(x[j], x[i])));
+  for (int i = 0; i < n; ++i) b[i] = P8_DADD(P8_DMUL(lambda, b[i]), P8_DMUL(one_minus, P8_DMUL(x[i], val)));
   km++;
-  if (km >= 4) {
-    for (int i = 0; i < OLS_N; ++i) for (int j = 0; j < OLS_N; ++j) ch[i * 32 + j] = cov[i * 32 + j];
-    for (int i = 0; i < OLS_N; ++i) ch[i * 32 + i] = P8_DADD(ch[i * 32 + i], nu);
+  if (km >= kmax) {
+    for (int i = 0; i < n; ++i) for (int j = 0; j < n; ++j) ch[i * n + j] = cov[i * n + j];
+    for (int i = 0; i < n; ++i) ch[i * n + i] = P8_DADD(ch[i * n + i], nu);
     bool fail = false;
-    for (int i = 0; i < OLS_N && !fail; ++i) {
+    for (int i = 0; i < n && !fail; ++i) {
       for (int j = 0; j < i; ++j) {
-        double sum = ch[i * 32 + j];
-        for (int k = 0; k < j; ++k) sum = P8_DSUB(sum, P8_DMUL(ch[i * 32 + k], ch[j * 32 + k]));
-        ch[i * 32 + j] = P8_DDIV(sum, ch[j * 32 + j]);
+        double sum = ch[i * n + j];
+        for (int k = 0; k < j; ++k) sum = P8_DSUB(sum, P8_DMUL(ch[i * n + k], ch[j * n + k]));
+        ch[i * n + j] = P8_DDIV(sum, ch[j * n + j]);
       }
-      double sum = ch[i * 32 + i];
-      for (int k = 0; k < i; ++k) sum = P8_DSUB(sum, P8_DMUL(ch[i * 32 + k], ch[i * 32 + k]));
-      if (sum > 1E-8) ch[i * 32 + i] = P8_DSQRT(sum); else fail = true;
+      double sum = ch[i * n + i];
+      for (int k = 0; k < i; ++k) sum = P8_DSUB(sum, P8_DMUL(ch[i * n + k], ch[i * n + k]));
+      if (sum > 1E-8) ch[i * n + i] = P8_DSQRT(sum); else fail = true;
     }
     if (!fail) {
-      for (int i = 0; i < OLS_N; ++i) {
+      for (int i = 0; i < n; ++i) {
         double sum = b[i];
-        for (int j = 0; j < i; ++j) sum = P8_DSUB(sum, P8_DMUL(ch[i * 32 + j], w[j]));
-        w[i] = P8_DDIV(sum, ch[i * 32 + i]);
+        for (int j = 0; j < i; ++j) sum = P8_DSUB(sum, P8_DMUL(ch[i * n + j], w[j]));
+        w[i] = P8_DDIV(sum, ch[i * n + i]);
       }
-      for (int i = OLS_N - 1; i >= 0; --i) {
+      for (int i = n - 1; i >= 0; --i) {
         double sum = w[i];
-        for (int j = i + 1; j < OLS_N; ++j) sum = P8_DSUB(sum, P8_DMUL(ch[j * 32 + i], w[j]));
-        w[i] = P8_DDIV(sum, ch[i * 32 + i]);
+        for (int j = i + 1; j < n; ++j) sum = P8_DSUB(sum, P8_DMUL(ch[j * n + i], w[j]));
+        w[i] = P8_DDIV(sum, ch[i * n + i]);
       }
     }
     km = 0;
   }
+}
+P8_HD inline double ols_predict(const double* blk, int n) {   // OLS::Predict() (:1446-1452); the caller resets the tap index
+  const double* x = blk; const double* w = blk + n;
+  double sum = 0.;
+  for (int i = 0; i < n; ++i) sum = P8_DADD(sum, P8_DMUL(w[i], x[i]));
+  return sum;
 }
 P8_HD inline void linear_predict(State& S) {   // Add() the new taps and Predict() (after the three Update() calls)
   LinearM& M = S.linear;
@@ -682,11 +690,8 @@ P8_HD inline void linear_predict(State& S) {   // Add() the new taps and Predict
       for (int k = 0; k < 3; ++k) if (M.ols_index[k] < OLS_N) M.ols[(size_t)k * OLS_STRIDE + M.ols_index[k]++] = (double)(u8)buf(S, idx[k]);
     }
     for (int k = 0; k < 3; ++k) {
-      double* x = M.ols + (size_t)k * OLS_STRIDE; double* w = x + 32;
       M.ols_index[k] = 0;
-      double sum = 0.;
-      for (int i = 0; i < OLS_N; ++i) sum = P8_DADD(sum, P8_DMUL(w[i], x[i]));
-      const double f = P8_FLOOR(sum);
+      const double f = P8_FLOOR(ols_predict(M.ols + (size_t)k * OLS_STRIDE, OLS_N));
       // Clip(int Px): the double is converted to int first (values far outside int range do not occur: |sum| < 2^20)
       M.prd[k] = (u8)clip8((int)f);
     }
@@ -704,22 +709,140 @@ P8_HD inline void linear_bit(State& S, Out& o) {
   LinearM& M = S.linear;
   if (S.bpos == 0) {
     const u8 W = (u8)buf(S, 1);
-    for (int k = 0; k < 3; ++k) ols_update(M.ols + (size_t)k * OLS_STRIDE, M.ols_km[k], W);
+    for (int k = 0; k < 3; ++k) ols_update(M.ols + (size_t)k * OLS_STRIDE, OLS_N, 4, 0.995, M.ols_km[k], (double)W);
     linear_predict(S);
   }
   for (int i = 0; i < 5; ++i) linear_small(S, o, i);
 }
 
+// ---------------------------------------------------------------- audio8bModel (:5552-5657), 8-bit PCM mono / stereo
+// At a byte boundary audio8b_begin does the scalar part (restart, channel, residuals of the sample just coded, the fixed
+// predictors), audio8b_ols(k) OLS predictor k: Update(s) on channel pCh = ch ^ stereo, then the taps and Predict() on
+// channel ch (independent of the other seven). Each bit audio8b_scm(q) is stationary map q = 3 * predictor + j.
+P8_HD inline int audio_ols_n(int k) { return k == 0 ? 128 : (k < 6 ? 90 : 28); }
+P8_HD inline int audio_ols_kmax(int k) { return k == 0 ? 24 : (k < 6 ? 29 + k : 10 - k); }
+P8_HD inline double audio_ols_lambda(int k) {
+  switch (k) {
+    case 0: return 0.9975; case 1: return 0.9965; case 2: return 0.996; case 3: case 4: return 0.995;
+    case 5: return 0.9985; case 6: return 0.98; default: return 0.992;
+  }
+}
+// blocks of 3n + 2n^2 doubles in the order (k, c): two of n = 128, ten of n = 90, four of n = 28
+enum { AUDIO_BLK128 = 3 * 128 + 2 * 128 * 128, AUDIO_BLK90 = 3 * 90 + 2 * 90 * 90, AUDIO_BLK28 = 3 * 28 + 2 * 28 * 28,
+       AUDIO_OLS_DOUBLES = 2 * AUDIO_BLK128 + 10 * AUDIO_BLK90 + 4 * AUDIO_BLK28 };
+P8_HD inline double* audio_ols_block(const AudioM& A, int k, int c) {
+  const int q = 2 * k + c;
+  const size_t off = k == 0 ? (size_t)c * AUDIO_BLK128
+                   : k < 6 ? 2 * (size_t)AUDIO_BLK128 + (size_t)(q - 2) * AUDIO_BLK90
+                           : 2 * (size_t)AUDIO_BLK128 + 10 * (size_t)AUDIO_BLK90 + (size_t)(q - 12) * AUDIO_BLK28;
+  return A.ols + off;
+}
+P8_HD inline bool audio8_mode(const State& S) { return S.detect.wav_info != 0 && ((S.detect.wav_info - 1) & 2) == 0; }
+// X1 / X2 (:5516-5542) for the two modes 8-bit data sets: wmode 0 (mono) and 1 (stereo; X2 only there)
+P8_HD inline int audio_x1(const State& S, int i) { return (S.audio->wmode ? buf(S, i << 1) : buf(S, i)) - 128; }
+P8_HD inline int audio_x2(const State& S, int i) { return buf(S, (i << 1) - 1) - 128; }
+P8_HD inline int sclip8(int v) { return imax(-128, imin(127, v)); }
+P8_HD inline void audio_add(AudioM& A, int k, double v) {   // OLS::Add / AddFloat on channel ch
+  int& idx = A.ols_index[k][A.ch];
+  if (idx < audio_ols_n(k)) audio_ols_block(A, k, A.ch)[idx++] = v;
+}
+P8_COLD P8_HD inline void audio8b_begin(State& S) {
+  AudioM& A = *S.audio;
+  const int info = (int)S.detect.wav_info - 1;
+  A.rpos = (S.pos == A.last_pos + 1) ? A.rpos + 1 : 0;
+  A.last_pos = S.pos;
+  if (A.rpos == 0) {
+    A.stereo = info & 1;
+    A.mask = 0;
+    S.st_record = ((u32)(A.stereo + 1) << 16) | (S.st_record & 0xFFFF);
+    A.wmode = info;
+  }
+  A.ch = A.stereo ? S.blpos & 1 : 0;
+  const int s = buf(S, 1) - 128, ch = A.ch, pch = ch ^ A.stereo;
+  u32 err = 0;
+  int i = 0;
+  for (; i < AUDIO_N_OLS; ++i) {
+    A.residuals[i][pch] = s - A.prd[i][pch][0];
+    const u32 r = (u32)iabs(A.residuals[i][pch]);
+    A.mask += A.mask + (r > 4);
+    err += r * r;
+  }
+  for (; i < AUDIO_N_PRD; ++i) A.residuals[i][pch] = s - A.prd[i][pch][0];
+  A.err_log = umin(0xF, ilog2(err));
+  A.mx_ctx = ilog2(umin(0x1F, bitcount(A.mask))) * 2 + (u32)ch;
+  const int x1 = audio_x1(S, 1), x2 = audio_x1(S, 2), x3 = audio_x1(S, 3), x4 = audio_x1(S, 4);
+  A.prd[8][ch][0] = sclip8(x1 * 2 - x2);
+  A.prd[9][ch][0] = sclip8(x1 * 3 - x2 * 3 + x3);
+  A.prd[10][ch][0] = sclip8(x1 * 4 - x2 * 6 + x3 * 4 - x4);
+  for (i = AUDIO_N_OLS; i < AUDIO_N_PRD; ++i) A.prd[i][ch][1] = sclip8(A.prd[i][ch][0] + A.residuals[i][pch]);
+}
+P8_HD inline void audio8b_taps(State& S, int k) {   // the Add() calls of predictor k, in the reference's order (:5599-5631)
+  AudioM& A = *S.audio;
+  const int st = A.stereo;
+  int i, j;
+  if (k >= 1 && k <= 5) {
+    const int k1 = 90, k2 = k1 - 12 * st;
+    if (k == 1) for (j = (i = 1); j <= k1; j++, i += 1 << ((j > 8) + (j > 16) + (j > 64))) audio_add(A, k, audio_x1(S, i));
+    if (k == 2) for (j = (i = 1); j <= k2; j++, i += 1 << ((j > 5) + (j > 10) + (j > 17) + (j > 26) + (j > 37))) audio_add(A, k, audio_x1(S, i));
+    if (k == 3) for (j = (i = 1); j <= k2; j++, i += 1 << ((j > 3) + (j > 7) + (j > 14) + (j > 20) + (j > 33) + (j > 49))) audio_add(A, k, audio_x1(S, i));
+    if (k == 4) for (j = (i = 1); j <= k2; j++, i += 1 + (j > 4) + (j > 8)) audio_add(A, k, audio_x1(S, i));
+    if (k == 5) for (j = (i = 1); j <= k1; j++, i += 2 + ((j > 3) + (j > 9) + (j > 19) + (j > 36) + (j > 61))) audio_add(A, k, audio_x1(S, i));
+    if (st && k >= 2 && k <= 4) for (i = 1; i <= k1 - k2; i++) audio_add(A, k, audio_x2(S, i));
+    return;
+  }
+  const int k1 = 28, k2 = k1 - 6 * st;
+  for (i = 1; i <= k2; i++) audio_add(A, k, audio_x1(S, i));
+  if (k == 0) for (; i <= 96; i++) audio_add(A, k, audio_x1(S, i));
+  if (st) {
+    for (i = 1; i <= k1 - k2; i++) audio_add(A, k, audio_x2(S, i));
+    if (k == 0) for (; i <= 32; i++) audio_add(A, k, audio_x2(S, i));
+  } else if (k == 0) for (; i <= 128; i++) audio_add(A, k, audio_x1(S, i));
+}
+P8_HD inline void audio8b_predict(State& S, int k, double sum) {   // Predict()'s result into the two predictions of k
+  AudioM& A = *S.audio;
+  const int ch = A.ch, pch = ch ^ A.stereo;
+  A.ols_index[k][ch] = 0;
+  A.prd[k][ch][0] = sclip8((int)P8_FLOOR(sum));
+  A.prd[k][ch][1] = sclip8(A.prd[k][ch][0] + A.residuals[k][pch]);
+}
+P8_HD inline void audio8b_ols(State& S, int k) {
+  AudioM& A = *S.audio;
+  const int n = audio_ols_n(k), pch = A.ch ^ A.stereo;
+  ols_update(audio_ols_block(A, k, pch), n, audio_ols_kmax(k), audio_ols_lambda(k), A.ols_km[k][pch], (double)(buf(S, 1) - 128));
+  audio8b_taps(S, k);
+  audio8b_predict(S, k, ols_predict(audio_ols_block(A, k, A.ch), n));
+}
+P8_HD inline void audio8b_scm(State& S, Out& o, int q) {
+  AudioM& A = *S.audio;
+  const int i = q / 3, j = q - 3 * i, bpos = S.bpos;
+  const int B = (int)(signed char)(u8)(S.c0 << (8 - bpos));
+  Scm& c = A.scm[i][j];
+  scm_set(c, (u32)((A.prd[i][A.ch][j == 2] - B) * 8 + bpos));
+  if (j == 2) scm_mix(c, o, S.y, 7, 1, 3);
+  else scm_mix(c, o, S.y, j == 0 ? 6 : 9, 1, 2 + (i >= AUDIO_N_OLS));
+}
+P8_HD inline void audio8b_select(State& S) {
+  const AudioM& A = *S.audio;
+  const int bpos = S.bpos, c0 = S.c0;
+  Mixer& m = S.m;
+  mset(m, (int)(A.err_log << 8) | c0, 4096);
+  mset(m, (int)(((A.mask & 0xFF) << 3) | ((u32)A.ch << 2) | (u32)(bpos >> 1)), 2048);
+  mset(m, (int)((A.mx_ctx << 7) | ((u32)buf(S, 1) >> 1)), 1280);
+  mset(m, (int)((A.err_log << 4) | ((u32)A.ch << 3) | (u32)bpos), 256);
+  mset(m, (int)A.mx_ctx, 10);
+}
+
 // ---------------------------------------------------------------- header detectors in front of the unmodelled image / audio / JPEG paths
 // The reference parses BMP / TGA / WAV / JPEG headers in ANY block and switches to dedicated models when one validates
-// (:5386-5509, :5810-5870, :5966-6060). Those models are not built; a validated header raises ERR_UNSUPPORTED_BLOCK.
+// (:5386-5509, :5810-5870, :5966-6060). Apart from 8-bit audio those models are not built; a validated header raises
+// ERR_UNSUPPORTED_BLOCK.
 P8_HD inline u32 le4(const State& S, int i) { return (u32)buf(S, i) + 256u * (u32)buf(S, i - 1) + 65536u * (u32)buf(S, i - 2) + 16777216u * (u32)buf(S, i - 3); }
 P8_HD inline int le2(const State& S, int i) { return buf(S, i) + 256 * buf(S, i - 1); }
 P8_HD inline u32 be4(const State& S, int i) { return (u32)buf(S, i - 3) + 256u * (u32)buf(S, i - 2) + 65536u * (u32)buf(S, i - 1) + 16777216u * (u32)buf(S, i); }
 // audioModel's parser (:5811-5866), run at the start of every byte: the WAVAudio header state, `length`, `eoi` and `info`.
 // info != 0 is audio mode: on those bytes the reference runs audio8bModel / wavModel and recordModel(AUDIO) instead of the
-// ordinary models. They are not built, so audio mode raises ERR_UNSUPPORTED_BLOCK; it starts on the first byte of a PCM data
-// chunk whose length is a whole number of sample blocks. Any other RIFF stream (AVI, WebP, compressed or 24-bit WAV,
+// ordinary models. audio8bModel is built (8-bit data, info 1 and 2); wavModel is not, so 16-bit audio mode raises
+// ERR_UNSUPPORTED_BLOCK. Audio mode starts on the first byte of a PCM data chunk whose length is a whole number of sample blocks. Any other RIFF stream (AVI, WebP, compressed or 24-bit WAV,
 // truncated headers, "RIFF" in text) codes with the ordinary models.
 P8_HD inline void wav_byte(State& S) {
   DetectM& D = S.detect;
@@ -754,7 +877,7 @@ P8_HD inline void wav_byte(State& S) {
     }
   }
   if (S.pos > (int)D.wav_eoi) D.wav_info = 0;
-  if (D.wav_info) S.error |= ERR_UNSUPPORTED_BLOCK;
+  if (D.wav_info && !audio8_mode(S)) S.error |= ERR_UNSUPPORTED_BLOCK;   // 16-bit audio mode only
 }
 P8_COLD P8_HD inline void detect_byte(State& S) {
   // JPEG: SOI followed by a plausible marker (:6046-6049)
@@ -907,6 +1030,15 @@ P8_HD inline int context_model(State& S) {
   rcm_mix(S.rcm9, o, c0, bpos);
   rcm_mix(S.rcm10, o, c0, bpos);
   match_bit(S, o);
+  if (audio8_mode(S)) {   // audioModel returns non-zero (:8167): audio8bModel, recordModel(AUDIO), and no other model
+    if (bpos == 0) { audio8b_begin(S); for (int k = 0; k < AUDIO_N_OLS; ++k) audio8b_ols(S, k); }
+    for (int q = 0; q < AUDIO_N_SCM; ++q) audio8b_scm(S, o, q);
+    audio8b_select(S);
+    record_core(S, o, S.rnd, FT_AUDIO);
+    record_select(S);
+    m.nx = o.n;
+    return mixer_predict(T, m, y, S.codes);
+  }
   const int ismatch = ilog(T, S.match.length);
   smatch_core(S, o);
   smatch_select(S);
@@ -918,7 +1050,7 @@ P8_HD inline int context_model(State& S) {
   if (bpos == 0) distance_byte(S);
   cm_mix(S.distance.cm, o, S.rnd, y, c0, bpos, buf(S, 1));
   pic_bit(S, o);
-  record_core(S, o, S.rnd);
+  record_core(S, o, S.rnd, S.filetype);
   record_select(S);
   record1_bit(S, o, S.rnd);
   if (bpos == 0) word_byte(S);

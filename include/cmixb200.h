@@ -24,7 +24,7 @@ extern "C" {
 
 enum { CMIXB200_OK = 0, CMIXB200_ERR_CUDA = 1, CMIXB200_ERR_ARG = 2,
        CMIXB200_ERR_CAPACITY = 3 /* a model arena is full (PPMD: raise CMIXB200_PPMD_MB); the stream is unusable */,
-       CMIXB200_ERR_UNSUPPORTED = 4 /* the resident PAQ8 met an image / PCM WAV audio / JPEG block it does not model; the stream is unusable */ };
+       CMIXB200_ERR_UNSUPPORTED = 4 /* the resident PAQ8 met an image / 16-bit PCM WAV audio / JPEG block it does not model; the stream is unusable */ };
 
 enum {
   CMIXB200_N_EXT = 2022,  /* replayed FXCM (431) + PAQ8 (1591) outputs per bit, as 12-bit codes k
@@ -41,8 +41,8 @@ void cmixb200_destroy(cmixb200_predictor*);
 
 /* Same, choosing which of the big model groups are REPLAYED instead of device resident: a replayed group costs no HBM
  * and takes its codes from cmixb200_feed_external_bit / the `ext` argument of the bulk calls; a bulk call without `ext`
- * gives its inputs p = 0.5. CMIXB200_REPLAY_PAQ8 is how image, PCM WAV audio and JPEG data are coded (the resident PAQ8
- * returns CMIXB200_ERR_UNSUPPORTED there). Predictors of one batch must replay the same groups, and decode_bytes needs
+ * gives its inputs p = 0.5. CMIXB200_REPLAY_PAQ8 is how image, 16-bit PCM WAV audio and JPEG data are coded (the resident
+ * PAQ8 returns CMIXB200_ERR_UNSUPPORTED there; it codes 8-bit PCM WAV audio itself). Predictors of one batch must replay the same groups, and decode_bytes needs
  * every group resident. cmixb200_create == replay_mask 0 == everything that is resident is used. */
 enum { CMIXB200_REPLAY_FXCM = 1, CMIXB200_REPLAY_PAQ8 = 2 };
 int cmixb200_create_ex(const uint8_t vocab[256], const char* dictionary_path, int device, unsigned replay_mask,
