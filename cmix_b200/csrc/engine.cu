@@ -271,6 +271,52 @@ int BuildSharedTablesLocked(int device, SharedTables& g_tables) {
   return CMIXB200_OK;
 }
 
+#ifdef CMIXB200_POISON
+// Poison build (poison.cuh): memory the code writes before it reads is filled with the pattern first, from a block of
+// the pattern per device. The device is idle around each fill: this is a test build.
+unsigned g_poison = POISON_DEFAULT;
+struct PoisonBlock { unsigned pattern; u8* p; };
+std::map<int, PoisonBlock> g_poison_block;
+const size_t kPoisonBytes = 16u << 20;
+
+cudaError_t PoisonSource(const u8** out) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  PoisonBlock& b = g_poison_block[dev];
+  if (e == cudaSuccess && (!b.p || b.pattern != g_poison)) {
+    if (b.p) cudaFree(b.p);
+    b.p = nullptr;
+    std::vector<u32> h(kPoisonBytes / 4);
+    for (size_t i = 0; i < h.size(); ++i) h[i] = poison_word(g_poison, (unsigned)i);
+    e = cudaMalloc(&b.p, kPoisonBytes);
+    if (e == cudaSuccess) e = cudaMemcpy(b.p, h.data(), kPoisonBytes, cudaMemcpyHostToDevice);
+    b.pattern = g_poison;
+  }
+  *out = b.p;
+  return e;
+}
+// rows of `width` bytes, `pitch` bytes apart
+cudaError_t PoisonFill2D(void* p, size_t pitch, size_t width, size_t rows) {
+  const u8* src = nullptr;
+  cudaError_t e = PoisonSource(&src);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  const size_t per = width ? kPoisonBytes / width : 0;
+  for (size_t r = 0; e == cudaSuccess && width && r < rows; r += per)
+    e = cudaMemcpy2D((u8*)p + r * pitch, pitch, src, width, width, std::min(per, rows - r), cudaMemcpyDeviceToDevice);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  return e;
+}
+cudaError_t PoisonFill(void* p, size_t bytes) {
+  const size_t rows = bytes / kPoisonBytes, tail = bytes % kPoisonBytes;
+  cudaError_t e = PoisonFill2D(p, kPoisonBytes, kPoisonBytes, rows);
+  if (e == cudaSuccess && tail) e = PoisonFill2D((u8*)p + rows * kPoisonBytes, tail, tail, 1);
+  return e;
+}
+#define POISON(...) __VA_ARGS__
+#else
+#define POISON(...) ((void)0)
+#endif
+
 // A device buffer that one predictor owns. Grow() replaces it by one of at least `count` elements (the contents are not kept)
 // and leaves it empty if the allocation fails; the buffer is freed when the predictor is deleted.
 template <class T> struct DeviceBuf {
@@ -285,7 +331,10 @@ template <class T> struct DeviceBuf {
     if (p) cudaFree(p);
     p = nullptr; n = 0;
     T* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, count * sizeof(T));
+    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
+#ifdef CMIXB200_POISON
+    if (e == cudaSuccess) e = PoisonFill(q, count * sizeof(T));
+#endif
     if (e == cudaSuccess) { p = q; n = count; }
     return e;
   }
@@ -342,6 +391,7 @@ struct cmixb200_predictor {
     void* q = nullptr;
     CK(cudaMalloc(&q, n * sizeof(T)));
     if (zero) CK(cudaMemset(q, 0, n * sizeof(T)));
+    else POISON(CK(PoisonFill(q, n * sizeof(T))));
     allocs.push_back(q);
     *p = (T*)q;
     return CMIXB200_OK;
@@ -683,6 +733,35 @@ std::pair<size_t, size_t> ReplayedSlots(const cmixb200_predictor* P) {
   return {P->d_fx ? (size_t)fx::N_OUT : 0, P->d_p8 ? (size_t)fx::N_OUT : (size_t)N_EXT};
 }
 
+#ifdef CMIXB200_POISON
+template <class T> cudaError_t PoisonBuf(DeviceBuf<T>& b) { return b.p ? PoisonFill(b.p, b.n * sizeof(T)) : cudaSuccess; }
+// The resident groups' slots of `rows` code rows: their kernels write every one before the mixer reads it.
+cudaError_t PoisonResident(const cmixb200_predictor* P, u16* codes, size_t rows) {
+  const size_t lo = P->d_fx ? 0 : (size_t)fx::N_OUT, hi = P->d_p8 ? (size_t)N_EXT : (size_t)fx::N_OUT;
+  return hi > lo ? PoisonFill2D(codes + lo, N_EXT * sizeof(u16), (hi - lo) * sizeof(u16), rows) : cudaSuccess;
+}
+// A bulk piece's per-bit scratch: the producers write each bit's inputs, selectors, PPMD rows, LSTM feedback and codes
+// before the mixer (or the next producer) reads them; the decay schedule is uploaded before the mixer reads it.
+int PoisonPiece(cmixb200_predictor* P) {
+  CK(PoisonBuf(P->d_small_x)); CK(PoisonBuf(P->d_sel)); CK(PoisonBuf(P->d_lstm_x)); CK(PoisonBuf(P->d_decay));
+  CK(PoisonBuf(P->d_lstm_fx)); CK(PoisonBuf(P->d_ppmd_gen));
+  if (P->d_ext_gen.p) CK(PoisonResident(P, P->d_ext_gen.p, P->d_ext_gen.n / N_EXT));
+  return CMIXB200_OK;
+}
+// Lock-step Predict(): the scratch it carries to Perceive() (StreamState, x .. small_x) is written by its kernels first.
+int PoisonPredict(cmixb200_predictor* P) {
+  CK(PoisonFill((u8*)P->d_st + offsetof(StreamState, x), offsetof(StreamState, ppmd) - offsetof(StreamState, x)));
+  return CMIXB200_OK;
+}
+// Lock-step Perceive(): the resident groups write every code of the next Predict(), and at the end of a byte with no
+// distribution fed, the PPMD model writes the distribution its consumers read.
+int PoisonPerceive(cmixb200_predictor* P, bool byte_done) {
+  CK(PoisonResident(P, P->d_ext_bit.p, 1));
+  if (byte_done && !P->ppmd_byte_valid) CK(PoisonBuf(P->d_ppmd_byte));
+  return CMIXB200_OK;
+}
+#endif
+
 // Launch the bulk kernels of one sub-chunk for a batch of streams whose ChunkArgs are already on the device:
 // ppmd -> (small | lstm -> fxcm) -> mix [-> encode], each on its own CUDA stream of the group's lead predictor.
 int LaunchChunk(cmixb200_predictor* lead, ChunkArgs* d_args, int n_streams, bool pretrain, bool with_coder = false,
@@ -785,6 +864,7 @@ int RunPipelined(cmixb200_predictor** preds, int n_streams, const u8* const* d_b
     TRY(SyncStreams(P));                                 // a lock-step Perceive() or the decoder may still be in flight
     if (!pretrain) TRY(EnsureScratch(P, n_bytes));      // Pretrain() touches models and contexts only: no per-bit scratch
     if (!pretrain && !(d_ppmd && d_ppmd[s])) CK(P->d_ppmd_gen.Grow(n_bytes * 256));
+    if (!pretrain) POISON(TRY(PoisonPiece(P)));
     if (!pretrain) {
       // the decay schedule depends only on the number of coded bits: streams that advance together share it
       // (393 216 double pow() calls per 2 KiB step and stream would otherwise cost more host time than a launch set)
@@ -999,6 +1079,7 @@ static int LaunchPredict(cmixb200_predictor* P) {
 
 float cmixb200_predict(cmixb200_predictor* P) {
   if (cudaSetDevice(P->device) != cudaSuccess) { g_last_error = "cudaSetDevice failed"; return -1.0f; }
+  POISON(if (PoisonPredict(P) != CMIXB200_OK) return -1.0f);
   if (LaunchPredict(P) != CMIXB200_OK) return -1.0f;
   float p = -1.0f;
   cudaError_t e = cudaMemcpyAsync(&p, &P->d_st->last_p, 4, cudaMemcpyDeviceToHost, P->s_mix);
@@ -1053,6 +1134,7 @@ int cmixb200_perceive(cmixb200_predictor* P, int bit) {
   bit = bit ? 1 : 0;
   const bool byte_done = P->bit_context >= 128;
   const u32 full = (P->bit_context * 2 + bit) & 255;
+  POISON(TRY(PoisonPerceive(P, byte_done)));
   // the previous Predict() waited for s_mix, so the row kernel that read d_ext_bit is done before PAQ8 rewrites its slots
   TRY(LaunchPerceive(P, bit, full, byte_done, MixerDecay(P->bits_done), nullptr));
   P->bits_done++;
@@ -1122,6 +1204,8 @@ int cmixb200_decode_bytes(cmixb200_predictor* P, const uint8_t* archive, size_t 
   auto fail = [&](const char* what) { g_last_error = std::string("decode_bytes: ") + what; r = CMIXB200_ERR_CUDA; };
   if (cudaMalloc(&d_arch, n_archive ? n_archive : 1) != cudaSuccess || cudaMalloc(&d_out, n_bytes) != cudaSuccess ||
       cudaMalloc(&d_decay, n_bits * sizeof(float)) != cudaSuccess) fail("out of device memory");
+  POISON(if (r == CMIXB200_OK && (PoisonFill(d_out, n_bytes) != cudaSuccess || PoisonPredict(P) != CMIXB200_OK ||
+                                  PoisonBuf(P->d_ppmd_byte) != cudaSuccess)) fail("poison fill failed"));
   if (r == CMIXB200_OK) {
     std::vector<float> decay;
     FillDecay(decay, P->bits_done, n_bits);
@@ -1193,6 +1277,7 @@ int cmixb200_code_bytes(cmixb200_predictor* P, const uint8_t* bytes, size_t n_by
   CK(P->d_ppmd.Grow(kSub * 256));
   for (size_t off = 0; off < n_bytes; off += kSub) {
     const size_t n = n_bytes - off < kSub ? n_bytes - off : kSub;
+    POISON(CK(PoisonBuf(P->d_bytes)); CK(PoisonBuf(P->d_p)); if (ext) CK(PoisonBuf(P->d_ext)); if (ppmd) CK(PoisonBuf(P->d_ppmd)));
     CK(cudaMemcpy(P->d_bytes.p, bytes + off, n, cudaMemcpyHostToDevice));
     if (ext) CK(cudaMemcpy(P->d_ext.p, ext + off * 8 * N_EXT, n * 8 * N_EXT * 2, cudaMemcpyHostToDevice));
     if (ppmd) CK(cudaMemcpy(P->d_ppmd.p, ppmd + off * 256, n * 256 * 4, cudaMemcpyHostToDevice));
@@ -1240,6 +1325,7 @@ int cmixb200_code_batch(cmixb200_predictor** preds, int n_streams, const uint8_t
     const size_t n = n_bytes - off < kSub ? n_bytes - off : kSub;
     for (int s = 0; s < n_streams; ++s) {
       cmixb200_predictor* P = preds[s];
+      POISON(CK(PoisonBuf(P->d_bytes2[k])); if (ext) CK(PoisonBuf(P->d_ext2[k])); if (ppmd) CK(PoisonBuf(P->d_ppmd2[k])));
       CK(cudaMemcpyAsync(P->d_bytes2[k].p, bytes[s] + off, n, cudaMemcpyHostToDevice, lead->s_copy));
       if (ext) CK(cudaMemcpyAsync(P->d_ext2[k].p, ext[s] + off * 8 * N_EXT, n * 8 * N_EXT * 2, cudaMemcpyHostToDevice, lead->s_copy));
       if (ppmd) CK(cudaMemcpyAsync(P->d_ppmd2[k].p, ppmd[s] + off * 256, n * 256 * 4, cudaMemcpyHostToDevice, lead->s_copy));
@@ -1255,6 +1341,7 @@ int cmixb200_code_batch(cmixb200_predictor** preds, int n_streams, const uint8_t
     CK(cudaStreamSynchronize(lead->s_copy));                      // stage(off) landed, previous results are on the host
     if (off + kSub < n_bytes) TRY(stage(off + kSub, k ^ 1));      // next inputs travel while this sub-step computes
     for (int s = 0; s < n_streams; ++s) {
+      POISON(CK(PoisonBuf(preds[s]->d_p)));
       db[s] = preds[s]->d_bytes2[k].p; de[s] = preds[s]->d_ext2[k].p; dp[s] = preds[s]->d_ppmd2[k].p; dout[s] = preds[s]->d_p.p;
     }
     const int rr = RunPipelined(preds, n_streams, db.data(), n, ext ? de.data() : nullptr, ppmd ? dp.data() : nullptr, dout.data(), false);
@@ -1273,6 +1360,7 @@ int cmixb200_coder_begin(cmixb200_predictor* P, size_t capacity_bytes) {
   if (capacity_bytes == 0) { g_last_error = "coder_begin: zero capacity"; return CMIXB200_ERR_ARG; }
   CK(P->d_code.Grow(capacity_bytes));
   CK(P->d_coder.Grow(1));
+  POISON(CK(PoisonBuf(P->d_code)));
   CoderState c; memset(&c, 0, sizeof c);
   c.x1 = 0; c.x2 = 0xffffffffu; c.cap = capacity_bytes; c.out = P->d_code.p;
   CK(cudaMemcpy(P->d_coder.p, &c, sizeof c, cudaMemcpyHostToDevice));
@@ -1362,6 +1450,20 @@ extern "C" int cmixb200_jitter_counts(unsigned* out, size_t n) {
     const cudaError_t e = get(out);
     if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return CMIXB200_ERR_CUDA; }
   }
+  return CMIXB200_OK;
+}
+#endif
+
+#ifdef CMIXB200_POISON
+// Poison build only (poison.cuh): the pattern of every later fill, of shared memory at each kernel's entry and of device
+// memory; set it before create. Not in include/cmixb200.h: a product build does not have it.
+namespace cmixb200 { POISON_MODULE(engine) }
+extern "C" int cmixb200_poison_config(unsigned pattern) {
+  for (auto set : {poison_set_engine, poison_set_fxcm, poison_set_paq8}) {
+    const cudaError_t e = set(pattern);
+    if (e != cudaSuccess) { g_last_error = cudaGetErrorString(e); return CMIXB200_ERR_CUDA; }
+  }
+  g_poison = pattern;
   return CMIXB200_OK;
 }
 #endif

@@ -22,6 +22,9 @@ JIT_MODULE(fxcm)
 #ifdef CMIXB200_CENSUS
 CENSUS_MODULE(fxcm)
 #endif
+#ifdef CMIXB200_POISON
+POISON_MODULE(fxcm)
+#endif
 
 }  // namespace cmixb200
 

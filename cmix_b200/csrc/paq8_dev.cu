@@ -22,6 +22,9 @@ JIT_MODULE(paq8)
 #ifdef CMIXB200_CENSUS
 CENSUS_MODULE(paq8)
 #endif
+#ifdef CMIXB200_POISON
+POISON_MODULE(paq8)
+#endif
 
 }  // namespace cmixb200
 

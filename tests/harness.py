@@ -56,16 +56,17 @@ def jitter_lib(tmp_path_factory):
 
 @pytest.fixture(scope="module")
 def ppmd_host(tmp_path_factory):
-    """tools/ppmd_host.cpp as a shared library: run(stream, vocab, arena_mb=64) -> (return code, [bytes][256] distributions)."""
+    """tools/ppmd_host.cpp as a shared library: run(stream, vocab, arena_mb=64, fill=0) -> (return code, [bytes][256]
+    distributions); fill: the byte every arena cell starts as (0: zeroed)."""
     lib = ctypes.CDLL(build_host_tool("ppmd_host", str(tmp_path_factory.mktemp("ppmd")), ["-shared", "-fPIC"]))
-    lib.ppmd_host_run.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint]
+    lib.ppmd_host_run.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint, ctypes.c_int]
     lib.ppmd_host_run.restype = ctypes.c_int
 
-    def run(stream, vocab, arena_mb=64):
+    def run(stream, vocab, arena_mb=64, fill=0):
         stream = np.ascontiguousarray(stream, dtype=np.uint8)
         vocab = np.ascontiguousarray(vocab, dtype=np.uint8)
         out = np.zeros((stream.size, 256), dtype=np.float32)
-        rc = lib.ppmd_host_run(stream.ctypes.data, stream.size, vocab.ctypes.data, out.ctypes.data, arena_mb)
+        rc = lib.ppmd_host_run(stream.ctypes.data, stream.size, vocab.ctypes.data, out.ctypes.data, arena_mb, fill)
         return rc, out
     return run
 
@@ -519,6 +520,14 @@ def child_jobs(jobs, run):
             break                        # the context may be gone: report, do not go on
 
 
+# every kernel of cmix_b200/csrc (each begins with jit_entry)
+KERNELS = ["fill_f32", "fill_u32", "fill_sse_rows", "fill_u16", "encode_kernel", "encode_flush_kernel", "decode_begin_kernel",
+           "decode_step_kernel", "fxcm_kernel", "fxcm_bit_kernel", "lstm_kernel", "lock_predict_inputs_kernel",
+           "lstm_byte_kernel", "mix_kernel_v3", "mix_predict_rows_kernel", "mix_predict_final_kernel", "mix_perceive_kernel",
+           "paq8_kernel", "paq8_bit_kernel", "ppmd_init_kernel", "ppmd_kernel", "ppmd_byte_kernel", "small_kernel",
+           "small_predict_kernel", "small_perceive_kernel"]
+
+
 def sass_by_function(path):
     """{function name: its SASS instructions} of a cubin or library (cuobjdump -sass; addresses and encodings dropped)."""
     text = subprocess.run(["cuobjdump", "-sass", path], check=True, capture_output=True, text=True).stdout
@@ -533,6 +542,15 @@ def sass_by_function(path):
             if ins:
                 funcs[name].append(ins)
     return {k: "\n".join(v) for k, v in funcs.items()}
+
+
+def sass_by_kernel(lib):
+    """{kernel name: its SASS}, the functions of a template kernel together."""
+    out = {}
+    for mangled, body in sass_by_function(lib).items():
+        name = next((k for k in KERNELS if re.search(r"\d%s[A-Z]" % k, mangled)), mangled)
+        out[name] = out.get(name, "") + body
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ the jitter build

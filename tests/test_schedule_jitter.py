@@ -19,16 +19,11 @@ import re
 
 import pytest
 
-from harness import CSRC, GROUPS, MAX_LINE, jitter_files, jitter_lib, run_jitter, sass_by_function  # noqa: F401  (jitter_lib: fixture)
+from harness import CSRC, GROUPS, KERNELS, MAX_LINE, jitter_files, jitter_lib, run_jitter, sass_by_kernel  # noqa: F401  (jitter_lib: fixture)
 
 SLOW = os.environ.get("CMIXB200_SLOW") == "1"
 SEEDS = [0x5EED0001, 0x5EED0002, 0x5EED0003]
 DENSITY = 16384                                   # random mode: a quarter of the visits sleep
-KERNELS = ["fill_f32", "fill_u32", "fill_sse_rows", "fill_u16", "encode_kernel", "encode_flush_kernel", "decode_begin_kernel",
-           "decode_step_kernel", "fxcm_kernel", "fxcm_bit_kernel", "lstm_kernel", "lock_predict_inputs_kernel",
-           "lstm_byte_kernel", "mix_kernel_v3", "mix_predict_rows_kernel", "mix_predict_final_kernel", "mix_perceive_kernel",
-           "paq8_kernel", "paq8_bit_kernel", "ppmd_init_kernel", "ppmd_kernel", "ppmd_byte_kernel", "small_kernel",
-           "small_predict_kernel", "small_perceive_kernel"]
 REACH = ["reach_english", "reach_europe", "reach_xml", "reach_x86", "reach_dbase", "reach_bmp", "reach_fxwiki"]
 WAV = "wav_pcm16_mono"
 
@@ -36,25 +31,16 @@ WAV = "wav_pcm16_mono"
 NEVER_FIRES = []
 
 
-def _sass_by_kernel(lib):
-    """{kernel name: its SASS}, the functions of a template kernel together."""
-    out = {}
-    for mangled, body in sass_by_function(lib).items():
-        name = next((k for k in KERNELS if re.search(r"\d%s[A-Z]" % k, mangled)), mangled)
-        out[name] = out.get(name, "") + body
-    return out
-
-
 def test_jitter_build_sleeps_in_every_kernel_and_the_product_nowhere(jitter_lib):
     import cmix_b200
-    jit = _sass_by_kernel(jitter_lib)
+    jit = sass_by_kernel(jitter_lib)
     missing = [k for k in KERNELS if k not in jit]
     assert not missing, "kernels not in the jitter build: %s" % missing
     quiet = [k for k in KERNELS if "NANOSLEEP" not in jit[k]]
     assert not quiet, "kernels of the jitter build without a sleep: %s" % quiet
     lib = ctypes.CDLL(jitter_lib)
     assert hasattr(lib, "cmixb200_jitter_config") and hasattr(lib, "cmixb200_jitter_counts")
-    prod = _sass_by_kernel(cmix_b200.build_library())
+    prod = sass_by_kernel(cmix_b200.build_library())
     assert sorted(prod) == sorted(jit), "the two builds hold different kernels"
     sleeping = [k for k, s in prod.items() if "NANOSLEEP" in s]
     assert not sleeping, "product kernels that sleep: %s" % sleeping

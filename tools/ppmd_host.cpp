@@ -8,20 +8,29 @@
 
 using namespace cmixb200;
 
+// An arena of n elements: zeroed (fill 0), or every byte `fill`, so that a read of a cell the model has not written
+// shows in its distribution.
+template <class T> static T* arena(size_t n, int fill) {
+  if (!fill) return (T*)calloc(n, sizeof(T));
+  T* p = (T*)malloc(n * sizeof(T));
+  if (p) memset(p, fill, n * sizeof(T));
+  return p;
+}
+
 extern "C" {
 
 // Runs the model over `stream` and writes PPMD::ByteUpdate's distribution after every byte (ppmd.cpp:1328-1338)
-// to out[n][256]. Returns 0, or 1 when the arenas (arena_mb in total) are exhausted.
-int ppmd_host_run(const unsigned char* stream, size_t n, const unsigned char* vocab, float* out, unsigned arena_mb) {
+// to out[n][256]. Returns 0, or 1 when the arenas (arena_mb in total, filled with the byte `fill`) are exhausted.
+int ppmd_host_run(const unsigned char* stream, size_t n, const unsigned char* vocab, float* out, unsigned arena_mb, int fill) {
   PpmdModel* m = new PpmdModel();
   memset(m, 0, sizeof *m);
   const size_t bytes = (size_t)arena_mb << 20;
   m->ctx_cap = (uint32_t)(bytes / 4 / sizeof(PpmdCtx));
   m->pool_cap = (uint32_t)(bytes / 2 / sizeof(PpmdSt));
   m->text_cap = (uint32_t)(bytes / 4);
-  m->ctx = (PpmdCtx*)calloc(m->ctx_cap, sizeof(PpmdCtx));
-  m->pool = (PpmdSt*)calloc(m->pool_cap, sizeof(PpmdSt));
-  m->text = (uint8_t*)calloc(m->text_cap, 1);
+  m->ctx = arena<PpmdCtx>(m->ctx_cap, fill);
+  m->pool = arena<PpmdSt>(m->pool_cap, fill);
+  m->text = arena<uint8_t>(m->text_cap, fill);
   ppmd_init(*m);
   int rc = 0;
   for (size_t t = 0; t < n && !rc; ++t) {
@@ -63,6 +72,6 @@ int main(int argc, char** argv) {
   std::vector<unsigned char> stream = slurp(argv[1]), vocab = slurp(argv[2]);
   if (stream.empty() || vocab.size() != 256) { fprintf(stderr, "ppmd_host: bad input\n"); return 2; }
   std::vector<float> out(stream.size() * 256);
-  return ppmd_host_run(stream.data(), stream.size(), vocab.data(), out.data(), 64);
+  return ppmd_host_run(stream.data(), stream.size(), vocab.data(), out.data(), 64, 0);
 }
 #endif
