@@ -5,15 +5,17 @@
 //    history maps on warps 7-8): bucket probe, bit-history step, state maps and the 5 / 7 mixer inputs of a context are
 //    independent of the other contexts of its map as long as they touch different 64-byte buckets this bit. That is CHECKED
 //    per bit (touched_buckets, including the buckets a deferred history write-back will reach; on the staying bits of the
-//    7-slot maps, bpos 1, 3, 4, 6, 7, the slots a context reads and writes, cm_slot_keys); a map with a clash is evaluated
-//    by one lane in the reference's order instead. On a staying bit a 7-slot lane reads its slot and run record from a
-//    copy in shared memory (P8CmCache).
+//    7-slot maps, bpos 1, 3, 4, 6, 7, the slots a context reads and writes, cm_slot_keys). In a 7-slot map with a clash
+//    only the contexts that share a key with another are evaluated by one lane in the reference's order (p8_number); a
+//    history map with a clash is evaluated by one lane whole. On a staying bit a 7-slot lane reads its slot and run record
+//    from a copy in shared memory (P8CmCache).
 //  * the one global coupling of the 7-slot maps, the shared pseudo-random sequence that ages high-count states
 //    (paq8.cpp:1075), is resolved between the two passes: the draws themselves depend on the generator only, so one warp
 //    computes as many as a bit can take during the bookkeeping, 24 at a time (the generator is a lagged XOR:
 //    x[i] = x[i-24] ^ x[i-55]); pass 1 computes each context's aged state and flags the contexts that draw; a flagged
 //    context's draw is the one its rank among the flagged contexts in program order selects (ballot masks + popcounts), and
-//    pass 2 applies them. A bit with a clashing map falls back to one lane walking the maps in order.
+//    pass 2 applies them. On a bit with a clashing map one lane first walks the contexts that share a key, setting their
+//    real flags, so that every rank counts final flags.
 //  * the match models, the DMC forest, the run maps and the direct maps run one unit per lane beside the context maps; on a
 //    bit inside a byte all of this is three phases (probe / number / apply), and the units take warps 9-11 and the text
 //    chain's idle warps 13-15, one function per warp and phase (lane map: P8_W_*). The bit that starts a byte
@@ -64,9 +66,11 @@ enum { P8_SEEN = 4096, P8_RING = 4 };
 // bit, each leg apart; not lane 0 on a bit with a clash, which walks the maps): probe 88 the state read, 89 touched_buckets,
 // 90 p8_claim; apply 91 the draw, 92 the store and the move to the next cell (bucket_find at bpos 2, 5, 0), 93 the run
 // record's input, 94 the cell's state and its StateMap load, 95 the other exports. On a staying bit leg 88 includes the
-// start of both StateMap loads and 94 also counts the probe's wait for them after p8_claim.
+// start of both StateMap loads and 94 also counts the probe's wait for them after p8_claim. By the bpos of a bit with a
+// 7-slot clash: 96 + bpos the numbering's cycles (p8_number and the barrier behind it), 104 + bpos the bits, 112 + bpos
+// the contexts it walked (grouped).
 #ifdef P8_PROF
-enum { P8_PROF_ROWS = 6, P8_PROF_SLOTS = 128, P8_PROF_UNIT = 64, P8_PROF_LEG = 88, P8_PROF_N = P8_PROF_SLOTS - 1 };
+enum { P8_PROF_ROWS = 6, P8_PROF_SLOTS = 128, P8_PROF_UNIT = 64, P8_PROF_LEG = 88, P8_PROF_NUMBER = 96, P8_PROF_N = P8_PROF_SLOTS - 1 };
 __device__ unsigned long long g_p8_prof[P8_PROF_ROWS][P8_PROF_SLOTS];
 #define P8_T(k) do { if (tid == 0) { const long long now_ = clock64(); atomicAdd(&sh.prof_dst[k], (unsigned long long)(now_ - sh.prof_t)); sh.prof_t = now_; } } while (0)
 #define P8_M0 const long long m0_ = clock64()
@@ -120,8 +124,9 @@ struct P8Slot {
 // Each 7-slot map lane's copy of the 7 state bytes of its slot (t[cp0 ..]) and the 2 bytes of its run record (t[runp ..]):
 // a staying bit (cm_staying) reads only these, so its probe and apply take them from shared memory. Stores go through to
 // HBM, which stays the authority. A copy is filled where the lane's bucket line is read anyway: after the lane's apply on a
-// move bit (bpos 0, 2, 5), or at the probe of a staying bit while it is invalid. It is valid from the fill until the map
-// walks serially (p8_number) or the launch ends: contexts without a clash never write another's slot or run record.
+// move bit (bpos 0, 2, 5), or at the probe of a staying bit while it is invalid. It is valid from the fill until the lane's
+// context is walked serially (p8_number) or the launch ends: a context never writes the slot or run record of a context it
+// shares no key with, and the walk writes only keys of the contexts it walks.
 struct P8CmCache {
   unsigned short sm[P8_CM_LANES][2];    // staying bit: smt[sm_cxt] and smt[the new cell's state], loaded by the probe
   unsigned char slot[P8_CM_LANES][8], run[P8_CM_LANES][2], valid[P8_CM_LANES];
@@ -145,9 +150,12 @@ struct P8Shared {
   int order, res2[P8_N_CM2];
   p8::WordStats snap;          // the word statistics as the byte found them (sparseModel1 reads them beside the word model's update)
   int dmc_st[10];
-  u32 flag_mask[8];            // ballot of "this context draws" per warp of map lanes
-  int flag_base[P8_N_CM];      // index of a map's first draw in draws[]
-  u32 draws[P8_CM_LANES + 6];  // the draws of the bit in order (p8_draw_seq); on a bit with a clash laid out by p8_number
+  u32 flag_mask[8];            // ballot of "this context draws" per warp of map lanes (p8_number sets the walked contexts' real flags)
+  u32 group_mask[8];           // on a bit with a clash: the lanes of clashing maps that share a key with another (p8_number)
+#ifdef CMIXB200_CENSUS
+  u32 flag_mask1[8];           // flag_mask as pass 1 left it: the census logs pass 1's flags
+#endif
+  u32 draws[P8_CM_LANES + 6];  // the draws of the bit in order (p8_draw_seq)
   int any_clash, text_pending;
   union {
     struct {                                                    // the model CTA
@@ -420,23 +428,47 @@ __device__ __noinline__ void p8_audio_ols_warp(P8Shared& sh, int k, int lane) {
 }
 
 // Insert the (map, bucket) pairs of one context into the per-bit set; returns true when a pair was already there, i.e. another
-// context of the same map touches the same 64-byte bucket this bit. A context's own repeats are removed first.
-__device__ bool p8_claim(unsigned long long* seen, int map, const u32* ids, int n) {
+// context of the same map touches the same 64-byte bucket this bit. A context's own repeats are removed first. A pair that
+// was already there is marked P8_KEY_SHARED, and ids[0..4] are replaced by the set's slots that hold the context's pairs
+// (n >= 1; the first one repeated past n), so that after the probe p8_shares tells whether the context met another.
+enum : unsigned long long { P8_KEY_SHARED = 1ull << 63 };
+__device__ bool p8_claim(unsigned long long* seen, int map, u32* ids, int n) {
   bool clash = false;
-  for (int a = 0; a < n; ++a) {
+  u32 slots[5];
+#pragma unroll
+  for (int a = 0; a < 5; ++a) {
+    if (a >= n) { slots[a] = slots[0]; continue; }
+    const u32 id = ids[a];
     bool dup = false;
-    for (int b = 0; b < a; ++b) dup = dup || ids[b] == ids[a];
-    if (dup) continue;
-    const unsigned long long key = ((unsigned long long)(map + 1) << 32) | ids[a];
-    u32 slot = (u32)((key * 0x9E3779B97F4A7C15ull) >> 52) & (P8_SEEN - 1);
-    for (;;) {
-      const unsigned long long old = atomicCAS(&seen[slot], 0ull, key);
-      if (old == 0ull) break;
-      if (old == key) { clash = true; break; }
-      slot = (slot + 1) & (P8_SEEN - 1);
+    u32 slot = 0;
+#pragma unroll
+    for (int b = 0; b < a; ++b) if (!dup && ids[b] == id) { dup = true; slot = slots[b]; }
+    if (!dup) {
+      const unsigned long long key = ((unsigned long long)(map + 1) << 32) | id;
+      slot = (u32)((key * 0x9E3779B97F4A7C15ull) >> 52) & (P8_SEEN - 1);
+      for (;;) {
+        const unsigned long long old = atomicCAS(&seen[slot], 0ull, key);
+        if (old == 0ull) break;
+        if ((old & ~P8_KEY_SHARED) == key) {
+          clash = true;
+          if (!(old & P8_KEY_SHARED)) atomicOr(&seen[slot], P8_KEY_SHARED);
+          break;
+        }
+        slot = (slot + 1) & (P8_SEEN - 1);
+      }
     }
+    slots[a] = slot;
   }
+#pragma unroll
+  for (int a = 0; a < 5; ++a) ids[a] = slots[a];
   return clash;
+}
+// after the probe's barrier: whether a context's pairs (the slots p8_claim left in ids) meet another context's
+__device__ __forceinline__ bool p8_shares(const unsigned long long* seen, const u32* slots) {
+  bool s = false;
+#pragma unroll
+  for (int a = 0; a < 5; ++a) s = s || (seen[slots[a]] & P8_KEY_SHARED) != 0;
+  return s;
 }
 
 // map (k, i) of a 7-slot-map lane, false if the lane is beyond the maps
@@ -548,6 +580,9 @@ __device__ __noinline__ void p8_probe_cm(P8Shared& sh, int tid, int y, int c0, i
   }
   const u32 mask = __ballot_sync(0xffffffffu, flag);
   if ((tid & 31) == 0) sh.flag_mask[tid >> 5] = mask;
+#ifdef CMIXB200_CENSUS
+  if ((tid & 31) == 0) sh.flag_mask1[tid >> 5] = mask;
+#endif
 }
 // the units that are one lane each, on the bit that starts a byte (warps 8-11 of the D-chain; record_pre and the linear
 // predictions' maps follow their models there)
@@ -595,24 +630,6 @@ __device__ __forceinline__ void p8_advance_rnd(P8Shared& sh, int lane) {
   for (int j = max(0, total - 64) + lane; j < total; j += 32) r.table[(i0 + 1 + j) & 63] = sh.draws[j];
   if (lane == 0) r.i = i0 + total;
 }
-// A bit in which two contexts of one 7-slot map meet in a bucket: one lane walks the maps in order, running the clashing ones
-// on the spot and laying out the draws of the others (draws[flag_base[k] + rank in map]).
-__device__ __noinline__ void p8_number(P8Shared& sh, int tid, int y, int c0, int bpos) {
-  using namespace p8;
-  State& S = sh.S;
-  if (tid != 0) return;
-  const int c1 = buf(S, 1);
-  int cur = 0;
-  for (int k = 0; k < P8_N_CM; ++k) {
-    Cm& m = p8_cm(S, k);
-    if (sh.clash[k]) { Out o = p8_out(sh, sh.unit_off[c_p8_cm_unit[k]]); cm_mix(m, o, S.rnd, y, c0, bpos, c1); }
-    else {
-      const int n = p8_flags_in(sh.flag_mask, c_p8_cm_base[k], c_p8_cm_base[k + 1]);
-      sh.flag_base[k] = cur;
-      for (int j = 0; j < n; ++j) sh.draws[cur++] = rnd_next(S.rnd);
-    }
-  }
-}
 // pass 2
 __device__ __noinline__ void p8_apply_cm2(P8Shared& sh, int tid, int y, int bpos, int maps) {
   int k, i;
@@ -628,18 +645,17 @@ __device__ __noinline__ void p8_apply_cm2(P8Shared& sh, int tid, int y, int bpos
 }
 __device__ __noinline__ void p8_apply_cm(P8Shared& sh, int tid, int y, int c0, int bpos) {
   using namespace p8;
-  const bool slow = sh.any_clash != 0;
-  if (!slow && tid < 32) p8_advance_rnd(sh, tid);      // flagged lanes read their draw from draws[], not from the table
+  if (tid < 32) p8_advance_rnd(sh, tid);      // flagged lanes read their draw from draws[], not from the table
   int k, i;
   if (!p8_cm_lane(tid, k, i)) return;
   Cm& m = p8_cm(sh.S, k);
   P8CmCache& cc = sh.u.md.cc;
-  if (sh.clash[k]) cc.valid[tid] = 0;      // lane 0 walks the map serially
-  if (sh.clash[k] || i >= m.cn) return;
+  if (sh.clash[k] && (sh.group_mask[tid >> 5] >> (tid & 31) & 1)) { cc.valid[tid] = 0; return; }   // walked by p8_number
+  if (i >= m.cn) return;
   P8_LEG(-1);
   int ns = sh.ns[tid];
   if (ns >= 204) {
-    const u32 r = sh.draws[slow ? sh.flag_base[k] + p8_flags_in(sh.flag_mask, c_p8_cm_base[k], tid) : p8_flags_in(sh.flag_mask, 0, tid)];
+    const u32 r = sh.draws[p8_flags_in(sh.flag_mask, 0, tid)];
     if (cm_draw_hits(r, ns)) ns -= 4;
   }
   P8_LEG(3);
@@ -845,9 +861,10 @@ static_assert(p8::N_IN % 8 == 0 && p8::N_IN / 8 <= 7 * 32, "a weight row is at m
 // first SGD warp waits for it (sync) and computes those sets beside the apply phase
 __device__ __forceinline__ void p8_signal_selects(int site) { jit_point(site); asm volatile("bar.arrive 2, 416;" ::: "memory"); }
 __device__ __forceinline__ void p8_await_selects(int site) { asm volatile("bar.sync 2, 416;" ::: "memory"); jit_point(site); }
-// named barrier 1 (warps 0-11): behind lane 0's numbering of a clashing bit and behind the apply phase, before lane 0's
-// epilogue reads res2 and clash; on the bit that starts a byte also between the probe and the numbering. Inside a byte the
-// unit warps 13-15 are not in it (nothing behind it reads their inputs before the bit's last __syncthreads)
+// named barrier 1 (warps 0-11): in a clashing bit's numbering (behind the grouped marks, behind lane 0's walk) and behind
+// the apply phase, before lane 0's epilogue reads res2 and clash; on the bit that starts a byte also between the probe and
+// the numbering. Inside a byte the unit warps 13-15 are not in it (nothing behind it reads their inputs before the bit's
+// last __syncthreads)
 __device__ __forceinline__ void p8_sync_maps(int site) { asm volatile("bar.sync 1, 384;" ::: "memory"); jit_point(site); static_assert(P8_MAP_THREADS == 384, "named barrier width"); }
 // The bit that starts a byte runs its context computation as independent chains of warps (p8_model_bit) ordered by three
 // more named barriers. Every arrive / sync below is executed by whole warps, unconditionally on that bit:
@@ -868,6 +885,48 @@ static_assert(P8_TID_MATCH == (P8_WARP_D + 2) * 32 && P8_TID_W10 == (P8_WARP_D +
 static_assert(P8_W_MATCH > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_SMATCH < (int)P8_MAP_WARPS && (int)P8_W_PIC == (int)P8_WARP_TEXT && (int)P8_W_RCM == (int)P8_WARPS - 1 &&
               P8_W_IMAP > (P8_CM2_TID0 + P8_CM2_LANES - 1) / 32 && (int)P8_W_DMCMIX < (int)P8_MAP_WARPS && (int)P8_W_SM32 == (int)P8_WARP_TEXT && (int)P8_W_STM == (int)P8_WARPS - 1,
               "barrier 3 inside a byte: the unit warps are 9-11 (in barriers 1 and 2 with the map warps) and 13-15 (in barrier 3 only)");
+
+// A bit on which two contexts of a 7-slot map meet (in a bucket on a move bit, in a slot on a staying bit), warps 0-11. A
+// context of a clashing map that shares a key with another is GROUPED; the others are FREE: nothing a grouped context writes
+// is a key of a free one, so a free context's aged state and flag from pass 1 stand and it runs in p8_apply_cm like a lane
+// of a clash-free map. Lane 0 walks the grouped contexts of all clashing maps in program order: each takes its aged state
+// from HBM as the earlier ones left it, sets its real flag in flag_mask and takes the draw of its rank, which counts the
+// final flags of every context before it (so the walk is one, not one per group or map). After it every flag is final.
+__device__ __noinline__ void p8_number(P8Shared& sh, int tid, int y, int c0, int bpos) {
+  using namespace p8;
+  State& S = sh.S;
+  int k, i;
+  const bool grouped = p8_cm_lane(tid, k, i) && sh.clash[k] && i < p8_cm(S, k).cn && p8_shares(sh.u.md.seen, sh.ids[tid]);
+  const u32 g = __ballot_sync(0xffffffffu, grouped);
+  if ((tid & 31) == 0 && tid < P8_CM2_TID0) sh.group_mask[tid >> 5] = g;
+  p8_sync_maps(JIT_HERE);
+  if (tid != 0) return;
+  const int c1 = buf(S, 1);
+#ifdef P8_PROF
+  int walked = 0;
+#endif
+  for (int w = 0; w < P8_CM2_TID0 / 32; ++w)
+    for (u32 gm = sh.group_mask[w]; gm; gm &= gm - 1) {
+      const int l = 32 * w + __ffs(gm) - 1;
+      p8_cm_lane(l, k, i);
+      Cm& m = p8_cm(S, k);
+      int ns = cm_next_state(*S.T, m, i, y);
+      const u32 bit = 1u << (l & 31);
+      if (ns >= 204) {
+        sh.flag_mask[w] |= bit;
+        if (cm_draw_hits(sh.draws[p8_flags_in(sh.flag_mask, 0, l)], ns)) ns -= 4;
+      } else sh.flag_mask[w] &= ~bit;
+      Out o = p8_out(sh, sh.unit_off[c_p8_cm_unit[k]] + 5 * i);
+      cm_step(m, i, o, ns, y, c0, bpos, c1);
+#ifdef P8_PROF
+      ++walked;
+#endif
+    }
+#ifdef P8_PROF
+  P8_C(P8_PROF_NUMBER + 8 + bpos, 1);
+  P8_C(P8_PROF_NUMBER + 16 + bpos, walked);
+#endif
+}
 
 // The mixer CTA's first bit in a new layout, on one warp: every cached row back to HBM, then the bit's sets fetched and their
 // dot products (no row is fetched before every row is written back, and no other warp reads them this bit)
@@ -1082,7 +1141,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       else p8_probe_cm2(sh, tid, bpos, 2);
       p8_sync_maps(JIT_HERE);
       P8_T(6);
-      if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(JIT_HERE); }
+      if (sh.any_clash) { P8_M0; p8_number(sh, tid, y, c0, bpos); p8_sync_maps(JIT_HERE); if (tid == 0) P8_M(P8_PROF_NUMBER + bpos); }
       P8_T(7);
       p8_apply_cm(sh, tid, y, c0, bpos);
       p8_apply_cm2(sh, tid, y, bpos, 2);
@@ -1104,7 +1163,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       p8_join_sync(JIT_HERE);
       p8_signal_selects(JIT_HERE);
       P8_T(3);
-      if (sh.any_clash) { p8_number(sh, tid, y, c0, bpos); p8_sync_maps(JIT_HERE); }
+      if (sh.any_clash) { P8_M0; p8_number(sh, tid, y, c0, bpos); p8_sync_maps(JIT_HERE); if (tid == 0) P8_M(P8_PROF_NUMBER + bpos); }
       P8_T(7);
       {
         P8_M0;
@@ -1121,7 +1180,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
     if (tid == 0) {
       P8_U0;
       if (bpos == 7) {
-        for (int k = 0; k < P8_N_CM; ++k) if (!sh.clash[k]) p8_cm(S, k).cn = 0;
+        for (int k = 0; k < P8_N_CM; ++k) p8_cm(S, k).cn = 0;
         for (int k = 0; k < P8_N_CM2; ++k) p8_cm2(S, k).index = 0;
       }
       if (!audio) main_select_fixed(S, sh.res2[0]);      // sets 19..27; warp 12 writes 0..18 (and the count) beside this
@@ -1130,7 +1189,7 @@ __device__ void p8_model_bit(P8Shared& sh, P8Slot* ring, u32 t, int y, int nb, i
       m.n2 = m.nx;
       while (m.nx & 7) m.tx[m.nx++] = 0;
       P8_U(23);
-      CENSUS_P8_BIT(S.sparse.cm.t, sh.clash, sh.clash2, sh.flag_mask, P8_CM_LANES, bpos);   // the bit's verdicts are final here
+      CENSUS_P8_BIT(S.sparse.cm.t, sh.clash, sh.clash2, sh.flag_mask1, P8_CM_LANES, bpos);   // the bit's verdicts are final here
 #ifdef P8_PROF
       prof_clash = sh.any_clash != 0;
 #endif

@@ -312,7 +312,8 @@ P8_HD inline void cm_set(Cm& m, u64 cx) {
   m.cn++;
 }
 // ---- ContextMap::mix1 (:1069-1145) cut per context, so that a CTA can run the contexts of a map side by side when they touch
-// disjoint buckets this bit (paq8.cuh) and fall back to the in-order loop (cm_mix) when they do not.
+// disjoint buckets this bit (paq8.cuh) and walk the contexts that share a bucket in order when they do not (p8_number;
+// cm_mix is the in-order loop of the host builds).
 // cm_next_state: the aged bit-history state context i would store this bit, BEFORE the random down-step (read-only); -1 = no cell.
 P8_HD inline int cm_next_state(const Tables& T, const Cm& m, int i, int y) { return m.cp[i] != P8_NULL ? T.state[m.t[m.cp[i]]][y] : -1; }
 P8_HD inline bool cm_draw_hits(u32 r, int ns) { return (u32)(r << ((452 - ns) >> 3)) != 0; }   // `rnd() << ((452-ns)>>3)` (:1075)

@@ -12,6 +12,9 @@
 //   clash7_bpos / bucket7_bpos       7-slot clash bits per bpos under the device's rule / under the bucket rule on every bit
 //   draw_bits, max_draws             bits with any draw of the shared sequence, the most draws in one bit
 //   gt24, gt24_fast                  bits with more than 24 draws; of those, bits without a 7-slot clash (the replay path)
+//   grouped, groups, group_max       in the clashing 7-slot maps: the contexts that share a key with another (the ones
+//                                    p8_number walks), their groups (contexts joined by shared keys, transitively) and the
+//                                    largest group; group_maps2 counts the map-bits with two or more groups
 // Include it before paq8_host.h / fxcm_host.h; call end_bit() after every bit and reset() after pretraining.
 //
 // Per-bit log (open_log; the census build of the device library writes the same words, paq8.cuh / fxcm.cuh CENSUS_*):
@@ -27,10 +30,14 @@
 // in-order rank, as the device's lanes do; cm2_mix_body; fxcm_model.h map_bit). If the rule is right, the codes stay the
 // reference's. "permuted" in the JSON line counts the map-bits whose order changed. -DCENSUS_REVERSE: the reverse order, on
 // the 7-slot maps' staying bits only.
+// -DCENSUS_GROUPS_PERMUTE=<seed>: every clashing 7-slot map as the device runs it (p8_number, p8_apply_cm), its free contexts
+// in a seeded pseudo-random order interleaved with the grouped ones (p8_cm_groups_order); "permuted" counts the map-bits whose
+// order changed.
 #pragma once
 #include <stdint.h>
 #include <stdio.h>
 
+#include <algorithm>
 #include <map>
 #include <set>
 #include <string>
@@ -45,6 +52,7 @@ struct Counts {
   uint32_t mask7 = 0, mask_bucket = 0, mask_hist = 0, mask_fx = 0, checked = 0;
   long bits = 0, draw_bits = 0, max_draws = 0, gt24 = 0, gt24_fast = 0, clash7_bits = 0, clash_hist_bits = 0, fx_clash_bits = 0;
   long clash7_stay = 0, clash7_bpos[8] = {}, bucket7_bpos[8] = {}, permuted = 0;
+  long grouped = 0, groups = 0, group_max = 0, group_maps2 = 0;
   std::map<const void*, long> p8_map;            // PAQ8 map -> bits with a clash in it
   std::map<int, long> fx_map;                    // FXCM map id -> bits with a clash in it
 };
@@ -79,14 +87,34 @@ inline bool claim(std::set<uint32_t>& seen, const uint32_t* ids, int n) {
 }
 
 inline bool staying(int bp) { return (0xDA >> bp) & 1; }     // cm_staying
-// p8_probe_cm's verdict for a 7-slot map: its contexts' slot keys on a staying bit, their buckets on the others
-template <class Map> bool p8_cm_clash(const Map& m, int c0, int bp) {
-  std::set<uint32_t> seen;
+inline int root(const int* grp, int i) { while (grp[i] != i) i = grp[i]; return i; }
+// The groups of a 7-slot map on this bit: contexts that share a key (p8_probe_cm's keys: slot keys on a staying bit, buckets
+// on the others) are joined, transitively. grp[i] = the first context of i's group, size[i] = the size of i's group. Returns
+// p8_probe_cm's verdict: whether any key is shared.
+template <class Map> bool p8_cm_groups(const Map& m, int c0, int bp, int* grp, int* size) {
+  std::map<uint32_t, int> first;            // key -> the first context that claimed it
   uint32_t ids[5];
   bool clash = false;
-  for (int i = 0; i < m.cn; ++i)
-    if (claim(seen, ids, staying(bp) ? cm_slot_keys(m, i, ids) : cm_touched(m, i, c0, bp, ids))) clash = true;
+  for (int i = 0; i < m.cn; ++i) grp[i] = i;
+  for (int i = 0; i < m.cn; ++i) {
+    const int n = staying(bp) ? cm_slot_keys(m, i, ids) : cm_touched(m, i, c0, bp, ids);
+    for (int a = 0; a < n; ++a) {
+      const auto r = first.emplace(ids[a], i);
+      if (r.second || r.first->second == i) continue;      // new, or the context's own repeat
+      clash = true;
+      const int x = root(grp, i), z = root(grp, r.first->second);
+      grp[x > z ? x : z] = x > z ? z : x;
+    }
+  }
+  for (int i = 0; i < m.cn; ++i) size[i] = 0;
+  for (int i = 0; i < m.cn; ++i) ++size[grp[i] = root(grp, i)];
+  for (int i = 0; i < m.cn; ++i) size[i] = size[grp[i]];
   return clash;
+}
+// p8_probe_cm's verdict for a 7-slot map
+template <class Map> bool p8_cm_clash(const Map& m, int c0, int bp) {
+  int grp[64], size[64];
+  return p8_cm_groups(m, c0, bp, grp, size);
 }
 // p8_probe_cm: every context i < cn claims its keys and flags a draw when its aged state is >= 204
 template <class Tab, class Map> void p8_cm(const Tab& T, const Map& m, int y, int c0, int bp) {
@@ -101,7 +129,19 @@ template <class Tab, class Map> void p8_cm(const Tab& T, const Map& m, int y, in
   C().bucket7 |= bucket;
   if (bucket) C().mask_bucket |= map_flag(&m);
   if (staying(bp)) C().checked += m.cn;
-  if (p8_cm_clash(m, c0, bp)) { C().clash7 = true; C().mask7 |= map_flag(&m); ++C().p8_map[&m]; }
+  int grp[64], size[64];
+  if (p8_cm_groups(m, c0, bp, grp, size)) {
+    C().clash7 = true; C().mask7 |= map_flag(&m); ++C().p8_map[&m];
+    int groups = 0;
+    for (int i = 0; i < m.cn; ++i) {
+      if (size[i] < 2) continue;
+      ++C().grouped;
+      if (grp[i] == i) ++groups;
+      if (size[i] > C().group_max) C().group_max = size[i];
+    }
+    C().groups += groups;
+    C().group_maps2 += groups >= 2;
+  }
 }
 
 #if defined(CENSUS_PERMUTE) || defined(CENSUS_REVERSE)
@@ -145,6 +185,59 @@ template <class Tab, class Map, class Out, class Rnd> int p8_cm_order(const Tab&
     result += cm_step(m, i, oi, s, y, c0, bp, c1);
   }
   o.n += 5 * m.cn;
+  if (bp == 7) m.cn = 0;
+  return result;
+}
+#endif
+#ifdef CENSUS_GROUPS_PERMUTE
+// cm_mix on a map the rule finds clashing, as the device runs it: the grouped contexts (those that share a key with another,
+// p8_number) in program order, each with the aged state and flag it finds when its turn comes; the free contexts (p8_apply_cm)
+// with the state and flag pass 1 computed, in a seeded pseudo-random order interleaved with the grouped ones. Each flagged
+// context takes the draw of its in-order rank among the final flags. That rank counts the flags of the grouped contexts before
+// it, so a flagged free context goes after those; an unflagged one goes anywhere. Returns cm_mix's result, or -1 where
+// cm_mix runs in order (a clash-free map).
+template <class Tab, class Map, class Out, class Rnd> int p8_cm_groups_order(const Tab& T, Map& m, Out& o, Rnd& rnd, int y, int c0, int bp, int c1) {
+  int grp[64], size[64];
+  if (!p8_cm_groups(m, c0, bp, grp, size)) return -1;
+  static uint64_t s = 0x9E3779B97F4A7C15ull ^ (uint64_t)(CENSUS_GROUPS_PERMUTE);
+  const int cn = m.cn;
+  int ns[64];
+  bool flag[64];
+  uint32_t draw[64];
+  Rnd r = rnd;
+  for (int j = 0; j < cn; ++j) draw[j] = rnd_next(r);          // the draw of each rank
+  // grouped context q (program order among them) at time 2q + 1, a free one at a random even time: 0 is before the first
+  // grouped context, 2G after the last; a flagged one not before 2 * (the grouped contexts before it)
+  std::vector<std::pair<uint64_t, int>> order;
+  int g = 0;
+  for (int i = 0; i < cn; ++i) g += size[i] > 1;
+  for (int i = 0, before = 0; i < cn; ++i) {
+    ns[i] = cm_next_state(T, m, i, y);
+    flag[i] = ns[i] >= 204;
+    s ^= s << 13; s ^= s >> 7; s ^= s << 17;
+    if (size[i] > 1) { order.push_back({(uint64_t)(2 * before + 1) << 32, i}); ++before; continue; }
+    const int lo = flag[i] ? before : 0;
+    const uint64_t gap = (uint64_t)lo + s % (uint64_t)(g - lo + 1);
+    order.push_back({(2 * gap) << 32 | (s >> 40), i});
+  }
+  std::sort(order.begin(), order.end());
+  for (int q = 0; q < cn; ++q) if (order[q].second != q) { ++C().permuted; break; }
+  int result = 0;
+  for (const auto& e : order) {
+    const int i = e.second;
+    int st = ns[i];
+    if (size[i] > 1) { st = cm_next_state(T, m, i, y); flag[i] = st >= 204; }
+    if (flag[i]) {
+      int rank = 0;
+      for (int j = 0; j < i; ++j) rank += flag[j];
+      if ((uint32_t)(draw[rank] << ((452 - st) >> 3)) != 0) st -= 4;   // cm_draw_hits
+    }
+    Out oi = o;
+    oi.n = o.n + 5 * i;
+    result += cm_step(m, i, oi, st, y, c0, bp, c1);
+  }
+  for (int i = 0; i < cn; ++i) if (flag[i]) rnd_next(rnd);
+  o.n += 5 * cn;
   if (bp == 7) m.cn = 0;
   return result;
 }
@@ -241,6 +334,8 @@ inline void print(FILE* f, const std::vector<std::pair<std::string, const void*>
   fprintf(f, "census {\"bits\": %ld, \"draw_bits\": %ld, \"max_draws\": %ld, \"gt24\": %ld, \"gt24_fast\": %ld, \"clash7\": %ld, "
              "\"clash7_stay\": %ld, \"clash_hist\": %ld, \"fx_clash\": %ld, \"permuted\": %ld, ", c.bits, c.draw_bits, c.max_draws,
           c.gt24, c.gt24_fast, c.clash7_bits, c.clash7_stay, c.clash_hist_bits, c.fx_clash_bits, c.permuted);
+  fprintf(f, "\"grouped\": %ld, \"groups\": %ld, \"group_max\": %ld, \"group_maps2\": %ld, ", c.grouped, c.groups, c.group_max,
+          c.group_maps2);
   const char* sep = "";
   for (const auto* v : {c.clash7_bpos, c.bucket7_bpos}) {
     fprintf(f, "\"%s\": [", v == c.clash7_bpos ? "clash7_bpos" : "bucket7_bpos");
@@ -263,6 +358,8 @@ inline void print(FILE* f, const std::vector<std::pair<std::string, const void*>
 #define P8_CENSUS_CM2(m, bpos) census::p8_cm2(m, bpos)
 #if defined(CENSUS_PERMUTE) || defined(CENSUS_REVERSE)
 #define P8_CM_ORDER(T, m, o, rnd, y, c0, bp, c1) do { const int r_ = census::p8_cm_order(T, m, o, rnd, y, c0, bp, c1); if (r_ >= 0) return r_; } while (0)
+#elif defined(CENSUS_GROUPS_PERMUTE)
+#define P8_CM_ORDER(T, m, o, rnd, y, c0, bp, c1) do { const int r_ = census::p8_cm_groups_order(T, m, o, rnd, y, c0, bp, c1); if (r_ >= 0) return r_; } while (0)
 #endif
 #ifdef CENSUS_PERMUTE
 #define P8_CM2_ORDER(m, o, y, bpos) do { const int r_ = census::p8_cm2_order(m, o, y, bpos); if (r_ >= 0) return r_; } while (0)

@@ -50,6 +50,12 @@ P8_LEGS = ["probe: state read", "probe: touched_buckets", "probe: p8_claim", "ap
            "apply: store and move (bucket_find at bpos 2, 5, 0)", "apply: run record input", "apply: cell state and StateMap load",
            "apply: other exports"]
 P8_LABELS.update({88 + k: "7-slot lane leg: " + s for k, s in enumerate(P8_LEGS)})
+# 96 + bpos: the numbering's cycles on the bits of that bpos with a 7-slot clash (p8_number: which contexts are grouped, the
+# walk of the grouped ones, the barrier behind it); 104 + bpos those bits; 112 + bpos the contexts walked on them
+P8_NUMBER = 96
+P8_LABELS.update({P8_NUMBER + b: "number on clashing bits, bpos %d" % b for b in range(8)})
+P8_LABELS.update({P8_NUMBER + 8 + b: "clashing bits, bpos %d" % b for b in range(8)})
+P8_LABELS.update({P8_NUMBER + 16 + b: "contexts walked, bpos %d" % b for b in range(8)})
 P8_ROWS, P8_SLOTS = 6, 128
 P8_CLASSES = ["byte boundary", "inside a byte", "same bucket", "same bucket, clash", "new bucket", "new bucket, clash"]
 
@@ -77,6 +83,12 @@ def paq8_classes(a):
         if any(a[r, k] for r in cols):
             print("  %-5d " % k + "".join("%19.0f" % (a[r, k] / n[r]) for r in cols) + "   " + P8_LABELS.get(k, ""))
     print("  %-5s " % "total" + "".join("%19.0f" % (a[r, :16].sum() / n[r]) for r in cols))
+    t = a[0] + a[1]
+    print("paq8 numbering on bits with a 7-slot clash, by bpos: bits, cycles per such bit, grouped contexts walked per such bit")
+    for b in range(8):
+        bits = t[P8_NUMBER + 8 + b]
+        if bits:
+            print("  bpos %d  %6d  %9.0f  %6.2f" % (b, bits, t[P8_NUMBER + b] / bits, t[P8_NUMBER + 16 + b] / bits))
 
 
 def build():
